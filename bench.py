@@ -1,10 +1,10 @@
 #!/usr/bin/env python
 """bench.py -- images/sec of the YOLOv5l semi-supervised (SSOD) training step @640, 16 labeled + 16 unlabeled per GPU.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl native|reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl native|reference] [--dump-outputs DIR]
   (N>1: python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 ... bench.py --gpus N ...)
 
-One "step" = SSODTrainerStep.train_instance: teacher-EMA forward on the unlabeled batch (native tcgen05 engine) ->
+One "step" = SSODTrainerStep.train_instance: teacher-EMA forward on the unlabeled batch (native wgmma engine) ->
 NMS + pseudo labels (native) -> student forward/backward on cat(labeled, strong-aug) -> ComputeLoss +
 ComputeStudentMatchLoss (native fused) -> gradient all-reduce (N>1) -> SGD-Nesterov -> both EMA updates (native fused).
 Nothing is skipped inside the timed region.  Prints ONE JSON line (rank 0).
@@ -12,9 +12,11 @@ Nothing is skipped inside the timed region.  Prints ONE JSON line (rank 0).
   value : images/s (B_l+B_u summed over ranks / max-over-ranks device time), inputs resident in HBM as fp32 [0,1]
   e2e   : same metric through the public step API from PINNED HOST uint8 batches: H2D copies + .float()/255 inside
           the timed region and a D2H read of the loss every step
-  roofline : dominant native kernel class = conv_fwd_kernel (tcgen05 implicit GEMM, teacher trunk): algorithmic conv
-          FLOPs of the teacher forward / CUDA-event time of the teacher_forward phase, vs the measured bf16 peak
+  roofline : dominant native kernel class = conv_fwd_kernel (wgmma implicit GEMM): algorithmic conv FLOPs / CUDA-event
+          time, vs the bf16 peak (MEASURED_PEAKS.json when present, else the H100 SXM data sheet)
   cpu_baseline : the oracle's CPU restatement of the same step (oracle/step_ref.py), bounded sample, rank 0, N=1 only
+--dump-outputs DIR writes what the last timed step computed (its loss, and a fixed seeded sample of the student's and the
+EMA teachers' weights after its optimizer / EMA updates) as DIR/<name>.npy, so two builds can be compared output for output.
 """
 import argparse
 import json
@@ -49,11 +51,12 @@ def peaks():
     try:
         return json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))), "measured"
     except Exception:
-        return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+        # NVIDIA H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense bf16 -- not measured, an upper bound
+        return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0}, "h100_sxm_datasheet"
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
 
     def __init__(self, index=0):
         super().__init__(daemon=True)
@@ -128,12 +131,11 @@ def conv_flops_teacher(engine_model, n_img, img):
 
 
 def dominant_kernel_roofline(dev, peak_tflops, peak_kind):
-    """The step's top kernel by GPU time (profiles/r1_step_kernel_table.md): conv_fwd2_kernel<256,6,0> -- the cta_group::2
-    tcgen05 implicit GEMM with the raw bf16 epilogue that runs the student's training forward AND (with transposed taps)
-    its dgrad -- on the shape family that carries 57% of the trunk FLOPs (3x3 s1 C->C Bottleneck conv; here 256->256 on
-    40x40 maps, batch 32 = the student's batch).  30 launches timed with CUDA events on the launching stream, rotating
-    over 6 input/output buffer sets (315 MB > the 126 MB L2) so no launch finds its input in L2.
-    Algorithmic FLOPs = 2*N*H*W*Cout*Cin*9; DRAM traffic from the committed ncu capture (profiles/r1_kernel_metrics.md)."""
+    """The conv kernel with the raw bf16 epilogue (conv_fwd_kernel<128,0>: the wgmma implicit GEMM that runs the student's
+    training forward AND, with transposed taps, its dgrad) on the shape family that carries 57% of the trunk FLOPs (3x3 s1
+    C->C Bottleneck conv; here 256->256 on 40x40 maps, batch 32 = the student's batch).  30 launches timed with CUDA events
+    on the launching stream, rotating over 6 input/output buffer sets (315 MB > the 50 MB L2) so no launch finds its input
+    in L2.  Algorithmic FLOPs = 2*N*H*W*Cout*Cin*9; algorithmic bytes = input + weights + output, each moved once."""
     from efficientteacher_b200 import convops as co
     N, H, C_ = 32, 40, 256
     nbuf = 6
@@ -154,19 +156,30 @@ def dominant_kernel_roofline(dev, peak_tflops, peak_kind):
     ms = s.elapsed_time(e) / n
     flops = 2.0 * N * H * H * C_ * C_ * 9
     ach = flops / ms / 1e9
-    return {"bound": "tensor", "kernel": "conv_fwd2_kernel<256,6,0> (cta_group::2 tcgen05 implicit GEMM, TMA-fed, raw bf16 epilogue: student forward + dgrad), 3x3 s1 256->256 @40x40, batch 32",
+    traffic = 2.0 * (2 * N * H * H * C_ + C_ * C_ * 9)
+    return {"bound": "tensor", "kernel": "conv_fwd_kernel<128,0> (wgmma implicit GEMM, TMA-fed, raw bf16 epilogue: student forward + dgrad), 3x3 s1 256->256 @40x40, batch 32",
             "achieved": ach, "peak": peak_tflops, "unit": "TFLOP/s", "frac": ach / peak_tflops,
-            "traffic": DOMINANT_TRAFFIC, "traffic_note": DOMINANT_TRAFFIC_NOTE,
+            "traffic": traffic, "traffic_note": "algorithmic bytes per launch (bf16 input + weights + output, no re-reads)",
             "peak_kind": peak_kind, "flops_per_launch": flops, "us_per_launch": ms * 1e3, "launches_timed": n,
             "l2": "rotating 6 buffer sets (315 MB) > L2"}
 
 
-# dram__bytes_read.sum + dram__bytes_write.sum per launch of the dominant kernel, from the committed ncu --set full capture
-DOMINANT_TRAFFIC = 27.47e6 + 0.11e6
-DOMINANT_TRAFFIC_NOTE = ("dram__bytes_read+write per launch from ncu --set full (profiles/r2_prof_conv_fwd2_raw_3x3_256_final.ncu-rep, 2 launches: "
-                         "27.47 MB read, 0.11 MB written: under ncu's serialised replay the 26.2 MB output stays L2-resident at kernel end; round "
-                         "1's capture with a cold L2 between launches showed 12.5-15.1 MB written); algorithmic bytes 26.2 MB in + 1.2 MB weights "
-                         "+ 26.2 MB out: no re-reads; tensor pipe 81.2 % active")
+DUMP_SAMPLE = 1 << 21      # weights sampled per model by --dump-outputs (8 MB of fp32 each)
+
+
+def dump_outputs(path, loss, models):
+    """--dump-outputs: the loss of the last timed step (float64) and, per model, the same fixed seeded sample of its floating
+    state (parameters + BN statistics, flattened in state_dict order) as it stands after that step (float32)."""
+    os.makedirs(path, exist_ok=True)
+    arrays = {"loss": loss.double().cpu().numpy().reshape(-1)}
+    idx = None
+    for name, m in models.items():
+        flat = torch.cat([v.detach().float().flatten() for v in m.state_dict().values() if v.is_floating_point()])
+        if idx is None:
+            idx = torch.randint(0, flat.numel(), (DUMP_SAMPLE,), generator=torch.Generator().manual_seed(1234)).sort().values
+        arrays[name + "_state_sample"] = flat[idx.to(flat.device)].cpu().numpy()
+    for k, v in arrays.items():
+        np.save(os.path.join(path, k + ".npy"), v)
 
 
 def kernel_table(step, ni, path, graph_ms):
@@ -251,8 +264,8 @@ def _best_threads(bl, bu):
 
 
 def run_reference(args, rank, world):
-    """--impl reference: the reference's CPU path of the step (oracle restatement; /root/reference cannot travel to the
-    GPU box).  Rank 0 only.  Each step = one full SSOD step on a bounded sample (2 labeled + 2 unlabeled images), fp32, with
+    """--impl reference: the reference's CPU path of the step (the oracle's restatement of the original
+    project's step, which needs none of its sources).  Rank 0 only.  Each step = one full SSOD step on a bounded sample (2 labeled + 2 unlabeled images), fp32, with
     the host thread count torch is fastest at (probed: all cores / 64 / 32 / 16)."""
     if rank != 0:
         return
@@ -359,7 +372,7 @@ def main():
     ap.add_argument("--impl", default="native", choices=["native", "reference"])
     ap.add_argument("--config", default="ssod640", choices=sorted(CONFIGS), help="ssod640 = the headline (BASELINE.json metric); ssod1280 / sup32 = configs[4] / configs[1]")
     ap.add_argument("--scaling", default="weak", choices=["weak", "strong"],
-                    help="weak (default, what the driver measures): the config's per-GPU batch at every N; strong: the config's batch is the "
+                    help="weak (default): the config's per-GPU batch at every N; strong: the config's batch is the "
                          "GLOBAL batch, split evenly over the ranks (SURVEY.md 8d: 16+16 -> 8+8 -> 4+4 -> 2+2 per GPU at 1/2/4/8 GPUs)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-eager-baseline", action="store_true")
@@ -368,6 +381,7 @@ def main():
     ap.add_argument("--allow-invalid", action="store_true", help="dev: print the line (marked invalid) even when the self-check fails")
     ap.add_argument("--nvtx-step", action="store_true", help="dev: wrap ONE extra eager step in the NVTX range 'etb_step' (ncu --nvtx --nvtx-include etb_step)")
     ap.add_argument("--kernel-table", default="", help="dev: write a per-kernel time table (torch.profiler/CUPTI, 2 eager steps) to this file")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR", help="write the last timed step's outputs as DIR/<name>.npy (see the module docstring)")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
@@ -536,14 +550,20 @@ def main():
         sampler.start()
     pl_probe = []
 
+    last_loss = []
+
     def step_resident_probed(i):          # device-side copies of the pseudo-label counters of the first / last timed step (no sync)
         out = step_resident(i)
+        if i == probe_last:
+            last_loss.append(out.clone())
         if ssod and (i == probe_first or i == probe_last):
             c = st.pseudo_label_creator
             pl_probe.append((c.last_count_dev.clone(), c.last_det[1].float().mean()))
         return out
     probe_first, probe_last = ni, ni + args.steps - 1
     ms = timed(step_resident_probed, args.steps, ni); ni += args.steps
+    if args.dump_outputs and rank == 0:      # before any further step moves the weights
+        dump_outputs(args.dump_outputs, last_loss[0], dict(student=st.model, teacher_ema=st.ema.ema, **({"semi_ema": st.semi_ema.ema} if ssod else {})))
     if ssod:
         probes = [(int(a.item()), float(b.item())) for a, b in pl_probe]
         (n_pl0, det_per_img0), (n_pl_timed, det_timed) = probes[0], probes[-1]        # --steps 1: first == last
@@ -637,8 +657,8 @@ def main():
             "config": {"workload": cb["workload"], "config_name": args.config,
                        "global_batch": imgs_per_step, "per_gpu_batch": [bl, bu], "img_size": img, "parallelism": "dp%d" % world, "grad_reduce": ("ncclAvg of the flat arena (reference: sum; see bench.py)" if world > 1 else "none (1 GPU)"), "cuda_graph": use_graph,
                        "schedule": "reference warm-up from ni=0 (nw=%s, nb=%d): lr/momentum change every step (device-resident hyper-parameters)" % (st.nw, NB),
-                       "l2": "inputs+activations per step (>1 GB) exceed the 126 MB L2; no explicit flush",
-                       "native": "teacher trunk+head, student conv fwd/dgrad/wgrad (tcgen05) + BatchNorm(train)+SiLU fwd/bwd, weight packing, NMS/pseudo-label, assigners, losses fwd/bwd, SGD, EMA",
+                       "l2": "inputs+activations per step (>1 GB) exceed the 50 MB L2; no explicit flush",
+                       "native": "teacher trunk+head, student conv fwd/dgrad/wgrad (wgmma) + BatchNorm(train)+SiLU fwd/bwd, weight packing, NMS/pseudo-label, assigners, losses fwd/bwd, SGD, EMA",
                        "self_check": health},
             "e2e": {"value": e2e_val, "unit": "images/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": 4, "ms_per_step": ms_e2e / args.steps},
             "gpu_launches": launches,

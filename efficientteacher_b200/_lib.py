@@ -185,7 +185,7 @@ def lib():
         if not os.path.exists(LIB_PATH):
             raise RuntimeError(
                 "libetb200.so not found at %s -- build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-                "(there is no CPU/PyTorch fallback for the B200 kernels)" % LIB_PATH)
+                "(there is no CPU/PyTorch fallback for the native kernels)" % LIB_PATH)
         _lib = C.CDLL(LIB_PATH)
         for name, (res, args) in _SIGS.items():
             fn = getattr(_lib, name)
@@ -201,7 +201,7 @@ def check(rc, what=""):
 
 def require_cuda(*tensors):
     if not torch.cuda.is_available():
-        raise RuntimeError("efficientteacher_b200 needs a CUDA (sm_100a) device: there is no CPU fallback")
+        raise RuntimeError("efficientteacher_b200 needs a CUDA (sm_90a) device: there is no CPU fallback")
     for t in tensors:
         if t is not None and not t.is_cuda:
             raise RuntimeError("expected a CUDA tensor, got %s" % (t.device,))

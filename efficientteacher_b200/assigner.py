@@ -41,7 +41,7 @@ class YOLOAnchorAssigner:
                  top_k=10):
         if num_keypoints or ota or single_targets:
             raise NotImplementedError("efficientteacher_b200: only build_targets / build_uc_targets_aug are on the "
-                                      "B200 hot path (SURVEY.md section 8 a9); OTA / keypoint / single-target "
+                                      "hot path (SURVEY.md section 8 a9); OTA / keypoint / single-target "
                                       "assigners are out of scope")
         self.na, self.nl, self.anchors, self.anchor_t = na, nl, anchors, anchor_t
         self.nc, self.np, self.stride, self.ota, self.top_k = nc, num_keypoints, stride, ota, top_k

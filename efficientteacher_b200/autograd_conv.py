@@ -1,4 +1,4 @@
-"""torch.autograd bridge for the tcgen05 convolutions: forward = implicit-GEMM conv, backward = dgrad (same kernel,
+"""torch.autograd bridge for the wgmma convolutions: forward = implicit-GEMM conv, backward = dgrad (same kernel,
 transposed taps) + wgrad (pixel-reduction GEMM).  Tensors stay NHWC bf16 in HBM and are exposed to torch as
 channels_last NCHW views (zero copy), so torch's BatchNorm/SiLU/cat/upsample/maxpool can sit between the convs while
 the dense contractions (97% of the step's FLOPs, SURVEY.md 8a a1) run on the hand-written kernels.
@@ -371,7 +371,7 @@ class ConvFn(torch.autograd.Function):
 
 class ConvBnActFn(torch.autograd.Function):
     """a = act(BatchNorm_train(conv2d(x, w))) -- the whole Conv module (common.py:480-481) in training mode:
-    tcgen05 conv -> per-channel batch statistics -> fused normalise+SiLU; backward = fused SiLU'/BN backward (2 passes)
+    wgmma conv -> per-channel batch statistics -> fused normalise+SiLU; backward = fused SiLU'/BN backward (2 passes)
     -> dgrad + wgrad.  Saves x, the raw conv output and [4,C] statistics (not the normalised tensor)."""
 
     @staticmethod
@@ -555,7 +555,7 @@ class DetectConvFn(torch.autograd.Function):
 
 class NetDFn(torch.autograd.Function):
     """netD behind GradReverse (models/detector/yolo_ssod.py:105-118,158-172,224-238): o = conv2(relu(conv1(x))) with the
-    gradient of x negated.  conv1 = tcgen05 GEMM with the ReLU in its epilogue; conv2 (C -> 2) = etb_netd_tail_fwd; the map is
+    gradient of x negated.  conv1 = wgmma GEMM with the ReLU in its epilogue; conv2 (C -> 2) = etb_netd_tail_fwd; the map is
     returned as an NCHW-shaped view [N,2,H,W] of the fp32 [N,H,W,2] buffer.  Backward: etb_netd_tail_bwd (dh with the ReLU
     mask, dW2 partials), conv1 wgrad into the arena, and conv1 dgrad on the NEGATED operand (pack mode 3) so the sign flip
     of GradReverse costs nothing and the result joins the feature's gradient fan-in."""

@@ -1,5 +1,5 @@
 """`import efficientteacher_b200.bootstrap` (first line of the reference's train.py / val.py, before its trainers are
-imported) rebinds the reference's hot-path symbols to the B200 mirrors -- see INTEGRATION.md section 1.  Requires the
+imported) rebinds the reference's hot-path symbols to the native mirrors -- see INTEGRATION.md section 1.  Requires the
 reference checkout on sys.path (it is the host application) and libetb200.so (no CPU fallback).
 
 The reference binds these symbols BY NAME with `from X import Y` in several places, and it loads some files twice under

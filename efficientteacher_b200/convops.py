@@ -1,4 +1,4 @@
-"""Thin Python wrappers over the tcgen05 convolution and the trunk layout kernels (NHWC bf16 tensors)."""
+"""Thin Python wrappers over the wgmma convolution and the trunk layout kernels (NHWC bf16 tensors)."""
 import ctypes as C
 import os
 
@@ -170,7 +170,7 @@ def conv_wgrad(x, dy, Cin, Cout, k, stride, pad, x_coffset=0, dy_coffset=0, stem
 # ---- training-mode BatchNorm + activation around the convs (csrc/bn.cu) ----
 # ETB_BN_FUSED=1: one cooperative launch per layer and direction (csrc/bn.cu bn_*_fused_kernel) instead of three kernels.
 # Opt-in: it removes 400 launches per step and its kernels are faster in isolation, but a cooperative grid needs the whole
-# GPU to itself, so it serialises against the weight-gradient side stream: 34.7 vs 32.2 ms/step (profiles/r2_ablation.md).
+# GPU to itself, so it serialises against the weight-gradient side stream (slower in the step).
 BN_FUSED = os.environ.get("ETB_BN_FUSED", "0") == "1"
 _bn_barriers = {}
 

@@ -1,4 +1,4 @@
-// bn.cu -- training-mode BatchNorm2d + SiLU around the tcgen05 convolutions, forward and backward (K1/K2 tails).
+// bn.cu -- training-mode BatchNorm2d + SiLU around the wgmma convolutions, forward and backward (K1/K2 tails).
 //   Conv.forward = act(bn(conv(x)))           reference models/backbone/common.py:480-481
 //   BN settings eps=1e-3, momentum=0.03       reference utils/torch_utils.py:162-171 (initialize_weights)
 // Replaces, per Conv, ATen's batch_norm_collect_statistics + batch_norm_transform_input + SiLU (5 passes over the

@@ -1,4 +1,4 @@
-// common.cuh -- shared helpers for libetb200 (sm_100a).  Compiled with --fmad=false: every fused
+// common.cuh -- shared helpers for libetb200 (sm_90a).  Compiled with --fmad=false: every fused
 // multiply-add in this library is an explicit fmaf()/__fmaf_rn so the bit-exact kernels (EMA, assigner,
 // NMS) reproduce the two-rounding arithmetic of the reference's CPU fp32 path.
 #pragma once
@@ -44,10 +44,10 @@ void etb_count_launch();   // every ETB_CHECK_LAUNCH() follows exactly one kerne
 // ETB_PDL_PROLOGUE(): `griddepcontrol.wait` (returns when the preceding kernel of the stream has completed and its memory is
 // visible -- so no kernel touches global data before its producer is done) followed by `griddepcontrol.launch_dependents`
 // (the NEXT kernel's CTAs may be scheduled as soon as all CTAs of this one have passed this point or exited).  The next
-// kernel's launch latency, block scheduling and prologue (smem carve-up, mbarrier init, TMEM allocation, tensor-map
-// prefetch: the tcgen05 kernels place the wait after that prologue) thereby overlap this kernel's execution instead of
-// following its tail.  Measured on the SSOD step: no gain once the step is replayed as a CUDA graph (the graph's kernel-to-kernel
-// latency is already ~1 us), so the attribute is only set with ETB_PDL=1 (eager-launch experiments).  A kernel launched without the attribute (ETB_PDL=0, or a neighbour from another library) sees both instructions
+// kernel's launch latency, block scheduling and prologue (smem carve-up, mbarrier init, tensor-map
+// prefetch: the conv kernels place the wait after that prologue) thereby overlap this kernel's execution instead of
+// following its tail.  Once the step is replayed as a CUDA graph the graph's kernel-to-kernel latency is already small,
+// so the attribute is only set with ETB_PDL=1 (eager-launch experiments).  A kernel launched without the attribute (ETB_PDL=0, or a neighbour from another library) sees both instructions
 // as no-ops / full stream order, so mixing is safe.  Captured CUDA graphs keep the programmatic edges.
 #define ETB_PDL_WAIT() asm volatile("griddepcontrol.wait;" ::: "memory")
 #define ETB_PDL_TRIGGER() asm volatile("griddepcontrol.launch_dependents;" ::: "memory")
@@ -61,7 +61,7 @@ static inline bool etb_pdl_enabled() {
   static int v = -1;
   if (v < 0) {
     const char* e = getenv("ETB_PDL");
-    v = (e && e[0] == '1') ? 1 : 0;       // opt-in: measured neutral under CUDA-graph replay (33.0 vs 32.8 ms/step, profiles/r2_ablation.md)
+    v = (e && e[0] == '1') ? 1 : 0;       // opt-in: eager-launch experiments
   }
   return v != 0;
 }
@@ -86,7 +86,7 @@ static inline int etb_num_sms() {
   if (!sms) {
     int dev = 0;
     if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0)
-      sms = 148;
+      sms = 132;   // H100 SXM
   }
   return sms;
 }

@@ -1,7 +1,7 @@
 // tail.cu -- the last library ops of the student's step, as native kernels (all HBM / latency bound, no tensor-core work):
 //   * Detect backward layout + bias gradient   reference models/head/yolov5_head.py:55,66 (the autograd of view/permute/
 //     contiguous + conv bias): fp32 loss gradient [N,na,H,W,no] -> bf16 NHWC dy [N,H,W,Cpad] (channel = a*no + o) for
-//     the tcgen05 dgrad / wgrad, and db[c] = sum over pixels in the same pass (two-stage, deterministic)
+//     the wgmma dgrad / wgrad, and db[c] = sum over pixels in the same pass (two-stage, deterministic)
 //   * netD tail                                 reference models/detector/yolo_ssod.py:224-238: conv2 (C -> 2, 1x1, no bias)
 //     on relu(conv1(x)) forward and backward (dh with the ReLU mask folded in, dW2 two-stage)
 //   * Domain / Target focal loss                reference models/loss/loss.py:312-421: 0.5 * mean(-(1-p)^2 log p),

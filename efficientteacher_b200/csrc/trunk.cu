@@ -1,4 +1,4 @@
-// trunk.cu -- layout / pooling / folding helpers around the tcgen05 convolutions (K3, K4, K18).
+// trunk.cu -- layout / pooling / folding helpers around the wgmma convolutions (K3, K4, K18).
 //   stem im2col + /255      reference trainer/ssod_trainer.py:694-696, models/backbone/yolov5_backbone.py:56
 //   SPPF max pools + concat reference models/backbone/common.py:702-708
 //   nearest 2x upsample     reference models/neck/yolov5_neck.py:92,97 (+ Concat common.py:796-797, free by slicing)

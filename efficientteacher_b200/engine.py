@@ -1,5 +1,5 @@
 """Native inference engine for the YOLOv5 trunk + Detect head: the teacher-EMA forward of the SSOD step
-(trainer/ssod_trainer.py:595-599 -> models/detector/yolo_ssod.py:105-118) on hand-written sm_100a kernels.
+(trainer/ssod_trainer.py:595-599 -> models/detector/yolo_ssod.py:105-118) on hand-written sm_90a kernels.
 
 Data layout: every activation is NHWC bf16 in HBM.  torch.cat never happens: producers write straight into the
 channel slice of the consumer's concat buffer (C3's [m(cv1(x)), cv2(x)], SPPF's [x,y1,y2,y3], the PANet concats),
@@ -60,7 +60,7 @@ class TrunkEngine:
                 self.params[d + ".conv1"].act = "relu"
         for q in self.params.values():
             if q.Cin % 8 != 0 and not q.stem:
-                raise NotImplementedError("tcgen05 conv path needs Cin %% 8 == 0 (16 B rows; got %d)" % q.Cin)
+                raise NotImplementedError("wgmma conv path needs Cin %% 8 == 0 (16 B rows; got %d)" % q.Cin)
         self.launches = 0
         self.packer = None
 

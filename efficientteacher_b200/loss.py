@@ -99,7 +99,7 @@ class ComputeLoss:
             raise NotImplementedError("fused loss supports pos_weight=1, no focal loss, no autobalance "
                                       "(the defaults of every shipped config)")
         if cfg.Loss.assigner_type == 'SimOTA':
-            raise NotImplementedError("OTA loss is not on the B200 hot path (use_ota=False in every shipped config)")
+            raise NotImplementedError("OTA loss is not on the hot path (use_ota=False in every shipped config)")
         self.cp, self.cn = smooth_BCE(eps=cfg.Loss.label_smoothing)
         det = model.module.head if is_parallel(model) else model.head
         self.balance = {3: [4.0, 1.0, 0.4]}.get(det.nl, [4.0, 1.0, 0.25, 0.06, .02])

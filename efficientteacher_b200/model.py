@@ -5,9 +5,9 @@ so reference checkpoints / EMA deep copies / optimizer param grouping keep worki
 
 Execution:
   * eval / no-grad forward (the teacher-EMA pass of trainer/ssod_trainer.py:595-599) runs on the native engine
-    (engine.TrunkEngine: tcgen05 implicit-GEMM convs, NHWC bf16, BN folded, concat-by-offset, fused Detect).
+    (engine.TrunkEngine: wgmma implicit-GEMM convs, NHWC bf16, BN folded, concat-by-offset, fused Detect).
   * training forward/backward: torch autograd only sequences the graph; every node is a native Function
-    (autograd_conv.ConvBnActFn = tcgen05 conv + fused BatchNorm(train)+SiLU(+shortcut), JoinFn / SppfPoolFn /
+    (autograd_conv.ConvBnActFn = wgmma conv + fused BatchNorm(train)+SiLU(+shortcut), JoinFn / SppfPoolFn /
     UpsampleIntoFn = concat-by-offset glue of csrc/glue.cu, DetectConvFn), tensors stay NHWC bf16 and are exposed to
     torch as channels_last views.
 There is no CPU path: forward raises without a CUDA device + libetb200.so.
@@ -54,7 +54,7 @@ class Conv(nn.Module):
         s.pop("_packed", None)
         return s
 
-    NATIVE = True        # training convs on the tcgen05 fwd/dgrad/wgrad kernels (False: torch/cuDNN scaffold)
+    NATIVE = True        # training convs on the wgmma fwd/dgrad/wgrad kernels (False: torch/cuDNN scaffold)
     FUSED_BN = True      # BatchNorm(train)+SiLU forward/backward on the fused kernels of csrc/bn.cu (False: torch ops)
     FUSED_GLUE = True    # concat-by-offset / fused shortcut add / native pool+upsample (csrc/glue.cu) instead of torch ops
     FUSED_FANIN = True   # gradient fan-in (C3 input, shortcut, backbone feature) accumulated in the dgrad epilogue
@@ -187,7 +187,7 @@ class YoloV5BackBone(nn.Module):
         d = lambda n: max(round(n * self.gd), 1) if n > 1 else n  # noqa: E731
         act = 'silu' if cfg.Model.Backbone.activation == 'SiLU' else None
         if act is None:
-            raise NotImplementedError("only SiLU YOLOv5 trunks are on the B200 hot path")
+            raise NotImplementedError("only SiLU YOLOv5 trunks are on the hot path")
         c1, c2, c3, c4, c5 = w(64), w(128), w(256), w(512), w(1024)
         self.stage1 = Conv(3, c1, 6, 2, 2, 1, act)
         self.stage1.is_stem = True
@@ -236,7 +236,7 @@ class YoloV5Neck(nn.Module):
         self.output_p3, self.output_p4, self.output_p5 = op3, op4, op5
         act = 'silu' if cfg.Model.Neck.activation == 'SiLU' else None
         if act is None:
-            raise NotImplementedError("only SiLU YOLOv5 trunks are on the B200 hot path")
+            raise NotImplementedError("only SiLU YOLOv5 trunks are on the hot path")
         self.conv1 = Conv(ip5, int(ip5 / 2), 1, 1, None, 1, act)
         self.upsample1 = nn.Upsample(scale_factor=2, mode="nearest")
         self.C1 = C3(int(ip5 / 2) + ip4, ip4, d(3), False, 1, 0.5, act)

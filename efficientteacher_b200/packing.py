@@ -1,4 +1,4 @@
-"""One-launch weight preparation for the tcgen05 convolutions.
+"""One-launch weight preparation for the wgmma convolutions.
 
 Every step the student's fp32 OIHW parameters change (SGD) and so does the teacher (EMA), so the bf16 K-major GEMM operands
 must be rebuilt: forward operand [Cout][kh*kw*Cin], dgrad operand per output-parity class [Cin][taps*Cout], stem operand

@@ -22,7 +22,7 @@ class FairPseudoLabel:
         self.names = cfg.Dataset.names
         self.num_points = cfg.Dataset.np
         if self.multi_label or self.num_points:
-            raise NotImplementedError("SSOD.multi_label / keypoints are not on the B200 hot path")
+            raise NotImplementedError("SSOD.multi_label / keypoints are not on the hot path")
         self.last_rows_dev = None
         self.last_count_dev = None
         self.last_det = None

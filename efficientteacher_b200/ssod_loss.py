@@ -40,7 +40,7 @@ class ComputeStudentMatchLoss:
         if not self.uncertain_aug:
             # the reference builds a single-target assigner for the *certain* set in this mode but still calls
             # build_uc_targets_aug for the others (ssod_loss.py:205-208); only uncertain_aug=True is shipped.
-            raise NotImplementedError("SSOD.uncertain_aug=False is not on the B200 hot path")
+            raise NotImplementedError("SSOD.uncertain_aug=False is not on the hot path")
         for k in 'na', 'nc', 'nl', 'anchors', 'stride':
             setattr(self, k, getattr(det, k))
         self.assigner = YOLOAnchorAssigner(self.na, self.nl, self.anchors, self.anchor_t, det.stride, self.nc,

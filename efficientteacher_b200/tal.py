@@ -8,7 +8,7 @@ Mirrors, with the reference's names and call contracts:
 
 The reference defines no end-to-end training step for this head (`models/loss/tal_loss.py` imports two modules that do not exist
 and `SSODTrainer.train_instance` raises for it), so these are standalone operators; the YOLOv8 trunk itself is not built (its
-channel widths -- 68, 192, 576 ... -- break the 8-channel vector contract of the tcgen05 conv kernels, DESIGN.md section 9).
+channel widths -- 68, 192, 576 ... -- break the 8-channel vector contract of the wgmma conv kernels, DESIGN.md section 9).
 There is no CPU fallback: every call needs libetb200.so and CUDA tensors.
 """
 import ctypes as C

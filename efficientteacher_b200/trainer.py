@@ -1,7 +1,7 @@
 """The SSOD training step with the reference's flow (trainer/ssod_trainer.py:587-680 train_instance,
 :458-488 update_optimizer, trainer/trainer.py:193-251 build_optimizer) for `model_type == 'yolov5'`:
 
-  teacher-EMA forward (native tcgen05 engine) -> NMS + pseudo labels (native, device resident) ->
+  teacher-EMA forward (native wgmma engine) -> NMS + pseudo labels (native, device resident) ->
   student forward on cat(labeled, strong-aug unlabeled) -> ComputeLoss + ComputeStudentMatchLoss (native fused
   fwd/bwd) -> backward -> [NCCL all-reduce of the student gradients] -> SGD-Nesterov -> ema / semi-ema update
   (native fused 5-stream kernel).
@@ -168,7 +168,7 @@ class SSODTrainerStep:
 
     # trainer/ssod_trainer.py:458-488 (bf16 autocast needs no GradScaler; loss scale == 1), in three parts so that the
     # gradient all-reduce can sit between two captured CUDA graphs when WORLD_SIZE > 1
-    WGRAD_SIDE_STREAM = os.environ.get("ETB_WGRAD_SIDE", "1") == "1"   # measured -0.9 ms/step (35.7 -> 34.9); ETB_WGRAD_SIDE=0 disables
+    WGRAD_SIDE_STREAM = os.environ.get("ETB_WGRAD_SIDE", "1") == "1"   # ETB_WGRAD_SIDE=0 disables
     TEACHER_SIDE_STREAM = os.environ.get("ETB_TEACHER_SIDE", "1") == "1"   # teacher forward + NMS concurrent with the student forward
 
     def _backward(self, loss):

@@ -1,5 +1,5 @@
 /*
- * etb200.h -- C ABI of libetb200.so, the B200 (sm_100a) kernels behind the EfficientTeacher SSOD step.
+ * etb200.h -- C ABI of libetb200.so, the H100 (sm_90a) kernels behind the EfficientTeacher SSOD step.
  *
  * The reference (AlibabaResearch/efficientteacher) is pure Python and has no FFI of its own
  * (SURVEY.md section 2.1), so every entry point below replaces a *library call made from Python*;
@@ -14,7 +14,7 @@
  *  - every launch goes to the stream passed in; nothing synchronises the device.
  *  - return value: 0 on success, negative errno-style code otherwise; etb_last_error() gives text.
  *    Errors are never thrown across the ABI.
- *  - there is NO CPU fallback: every compute entry point returns ETB_ERR_CUDA if no sm_100 device
+ *  - there is NO CPU fallback: every compute entry point returns ETB_ERR_CUDA if no sm_90 device
  *    kernel image can run.
  */
 #ifndef ETB200_H_
@@ -202,8 +202,8 @@ int etb_loss_backward(const float* const* p, float* const* grad_p, const EtbLoss
 
 /* ---------------------------------------------------------------------------------------------
  * Conv trunk (models/backbone/common.py:471-484 Conv = conv2d(bias=False)+BN+SiLU; Bottleneck :534-544;
- * models/head/yolov5_head.py:55 Detect 1x1).  tcgen05 implicit GEMM, NHWC bf16 operands, fp32 accumulate
- * in TMEM, TMA-fed.  x [N,H,W,Cin] bf16 (channel stride x_cstride >= Cin so a concat slice can be read in
+ * models/head/yolov5_head.py:55 Detect 1x1).  wgmma implicit GEMM, NHWC bf16 operands, fp32 accumulate
+ * in registers, TMA-fed.  x [N,H,W,Cin] bf16 (channel stride x_cstride >= Cin so a concat slice can be read in
  * place), w [Cout, kh*kw*Cin] bf16 (K-major), y [N,Ho,Wo,*] bf16 written at channel offset into a buffer
  * with y_cstride channels (so concat is free).
  *   epilogue: v = acc*scale[c] + bias[c]  (folded eval-mode BN, or conv bias with scale=NULL)
@@ -225,7 +225,7 @@ int etb_conv_fwd(const void* x_bf16, const void* w_bf16, const float* scale, con
                  void* workspace, size_t workspace_bytes, void* stream);
 
 /* data gradient of the same convolution (autograd of Conv.forward, SURVEY.md K2): dx = conv_transpose(dy, W), run as
- * implicit GEMMs on the same tcgen05 kernel -- one launch per output-parity class (1 for stride 1, 4 for stride 2).
+ * implicit GEMMs on the same wgmma kernel -- one launch per output-parity class (1 for stride 1, 4 for stride 2).
  * `cp` describes the FORWARD conv; cp->x_cstride is the channel stride of dy, cp->y_cstride / y_coffset place dx.
  * wd = etb_pack_weight_dgrad(w) (etb_dgrad_weight_elems bf16 elements).  accumulate != 0: dx += result. */
 int64_t etb_dgrad_weight_elems(int32_t Cout, int32_t Cin, int32_t k, int32_t stride);
@@ -234,7 +234,7 @@ int etb_pack_weight_dgrad(const float* w_oihw, void* out_bf16, int32_t Cout, int
 int etb_conv_dgrad(const void* dy_bf16, const void* wd_bf16, void* dx_bf16, const EtbConvParams* cp, int32_t accumulate,
                    void* stream);
 
-/* weight gradient (SURVEY.md K2): dW[co][tap][ci] = sum_pixels dy * x(shifted): tcgen05 GEMM with the pixels as the
+/* weight gradient (SURVEY.md K2): dW[co][tap][ci] = sum_pixels dy * x(shifted): wgmma GEMM with the pixels as the
  * reduction dimension (MN-major operands straight from the NHWC tensors via TMA).  Two-stage split-K: every CTA stores its
  * partial tile into its slice of `workspace`, then a reduce kernel sums the slices, converts to the parameter layout
  * [Cout,Cin,kh,kw] and writes (flags bit1: adds into) dw_f32 -- which may be the gradient-arena slice of the parameter.
@@ -340,7 +340,7 @@ int etb_pack_stem_weight(const float* w_oihw, void* w_bf16, int32_t Cout, void* 
 /* ---- the last library ops of the student's step (csrc/tail.cu) ----------------------------------------------------------
  * Detect backward layout: the fused loss hands back d(loss)/d(logits) as fp32 [N,na,H,W,no] (the train layout of
  * models/head/yolov5_head.py:66).  etb_detect_dy_pack rewrites it as the bf16 NHWC operand dy [N,H,W,Cpad] (channel =
- * a*no + o, pad channels zeroed) of the tcgen05 dgrad / wgrad and emits per-block column sums; etb_column_sum reduces them
+ * a*no + o, pad channels zeroed) of the wgmma dgrad / wgrad and emits per-block column sums; etb_column_sum reduces them
  * to the conv-bias gradient (yolov5_head.py:55: nn.Conv2d(..., bias=True)) -- replaces autograd's permute/contiguous/sum.
  * partials: [etb_detect_dy_rows(N,H,W)][na*no] floats. */
 int64_t etb_detect_dy_rows(int32_t N, int32_t H, int32_t W);

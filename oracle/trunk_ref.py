@@ -1,7 +1,7 @@
 """TEST INFRASTRUCTURE ONLY -- plain PyTorch fp32 functional forward of the YOLOv5 trunk + Detect + netD from a
 state_dict with the reference's key names (models/backbone/yolov5_backbone.py:76-88, models/neck/yolov5_neck.py:88-109,
 models/head/yolov5_head.py:47-87, models/detector/yolo_ssod.py:105-118, models/backbone/common.py Conv/Bottleneck/C3/SPPF).
-It is the torch reference the tcgen05 trunk is compared with, and the trunk of the CPU baseline in bench.py.
+It is the torch reference the wgmma trunk is compared with, and the trunk of the CPU baseline in bench.py.
 Works on any device; train=True uses batch statistics and, with bn_momentum > 0, updates the running statistics in the
 state_dict in place like nn.BatchNorm2d does (default 0: leaves them alone)."""
 import torch

@@ -12,7 +12,7 @@ GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA (B200) device; run on the GPU box with -m gpu")
+    config.addinivalue_line("markers", "gpu: needs a CUDA (H100) device; run on the GPU box with -m gpu")
 
 
 @pytest.fixture(scope="session")

@@ -1,4 +1,4 @@
-"""GPU (B200): the native teacher engine (tcgen05 trunk + Detect, NHWC bf16, folded BN, concat-by-offset) against the
+"""GPU (H100): the native teacher engine (wgmma trunk + Detect, NHWC bf16, folded BN, concat-by-offset) against the
 plain PyTorch fp32 forward of the same weights (oracle/trunk_ref.py, itself bit-identical to the reference modules),
 and one whole SSOD step against the oracle's CPU step."""
 import numpy as np
@@ -96,7 +96,7 @@ def test_full_ssod_step_runs_and_matches_cpu_step(img, bl, bu):
 
 
 def test_native_training_convs_vs_fp32_reference():
-    """Student forward/backward with every trunk/head conv on the tcgen05 fwd/dgrad/wgrad kernels (bf16 autocast).
+    """Student forward/backward with every trunk/head conv on the wgmma fwd/dgrad/wgrad kernels (bf16 autocast).
     At random init with a tiny batch the parameter gradients of ANY bf16 implementation only correlate ~0.8 with fp32
     (tools/debug_grad_noise.py: native 0.81, torch/cuDNN bf16 0.77), so the criterion is: against an fp32 (TF32 off) torch
     reference of the same step the native path is at least as accurate as the library bf16 path, per parameter; the

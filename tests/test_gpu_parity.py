@@ -1,4 +1,4 @@
-"""GPU (B200): the CUDA kernels, called through the reference-shaped Python mirrors over the C ABI, against the
+"""GPU (H100): the CUDA kernels, called through the reference-shaped Python mirrors over the C ABI, against the
 oracle (oracle/port.py) and the golden vectors of the live reference.  Bit-exact for indices / keep-sets / EMA;
 fp32 losses within 1e-4 relative (the tolerance BASELINE.json's north_star states)."""
 import math

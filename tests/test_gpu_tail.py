@@ -1,4 +1,4 @@
-"""GPU (B200): the native tail of the student's step (csrc/tail.cu) against plain PyTorch references of the same ops:
+"""GPU (H100): the native tail of the student's step (csrc/tail.cu) against plain PyTorch references of the same ops:
 Detect backward layout + bias gradient, netD tail (C -> 2) forward/backward, Domain/Target focal loss forward/backward
 (also against the oracle's restatement of models/loss/loss.py:312-421), the uint8 stem loader, and the zero-copy batch split."""
 import numpy as np

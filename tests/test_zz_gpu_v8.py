@@ -1,10 +1,9 @@
-"""GPU (B200): the anchor-free (YOLOv8 / TAL) operators of csrc/tal.cu through their reference-shaped mirrors
+"""GPU (H100): the anchor-free (YOLOv8 / TAL) operators of csrc/tal.cu through their reference-shaped mirrors
 (efficientteacher_b200/tal.py) against the golden vectors of the live reference and the oracle (oracle/port_v8.py).
 Labels / boxes / foreground masks bit-exact; target_scores within 1e-5 relative (the alignment metric goes through pow);
 decoded boxes within 1e-5 relative.
 
-This file sorts last on purpose: it was written when 5 GPU-minutes of the round were left (first B200 run: 11 passed,
-profiles/r2_v8_gpu_tests.log), and a failure here must never hide the results of the older suite before it (pytest -x)."""
+This file sorts last on purpose: a failure here must never hide the results of the older suite before it (pytest -x)."""
 import os
 
 import numpy as np

@@ -17,7 +17,7 @@ def main():
     from tools.conv_bench import timeit
     dev = "cuda:0"
     lib = _lib.lib()
-    pk = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"] if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else 6650.0
+    pk = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"] if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else 3350.0   # H100 SXM data sheet
     for (N, H, C_) in ((32, 320, 64), (32, 160, 64), (32, 160, 128), (32, 80, 128), (32, 80, 256), (32, 40, 256), (32, 40, 512), (32, 20, 512), (32, 20, 1024)):
         M = N * H * H
         y = torch.randn(N, H, H, C_, device=dev).to(torch.bfloat16)

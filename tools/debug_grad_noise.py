@@ -1,4 +1,4 @@
-"""Diagnostic: parameter-gradient agreement of (a) native tcgen05 convs under bf16 autocast and (b) torch/cuDNN under bf16
+"""Diagnostic: parameter-gradient agreement of (a) native wgmma convs under bf16 autocast and (b) torch/cuDNN under bf16
 autocast, each against an fp32 (no autocast, TF32 off) torch reference of the same step."""
 import os
 import sys

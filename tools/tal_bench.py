@@ -36,7 +36,8 @@ def main():
     from efficientteacher_b200 import _lib, tal
     dev = torch.device("cuda:0")
     torch.cuda.set_device(dev)
-    peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
+    pk_path = os.path.join(ROOT, "MEASURED_PEAKS.json")
+    peaks = json.load(open(pk_path)) if os.path.exists(pk_path) else {"hbm_gbs": 3350.0}   # H100 SXM data sheet
     out = {"hbm_peak_gbs": peaks["hbm_gbs"], "iters": args.iters, "cases": {}}
     B, img, nc = 32, 640, 80
     A = sum(h * w for h, w in synth.level_shapes(img))
