@@ -602,12 +602,16 @@ extern "C" int etb_conv_dgrad(const void* dy_bf16, const void* wd_bf16, void* dx
       memset(&ka, 0, sizeof(ka));
       signed char kh_l[12], kw_l[12];
       const int nt = dgrad_taps(k, s, pad, ph, pw, kh_l, kw_l, ka.tap_dh, ka.tap_dw);
+      // etb_pack_weight_dgrad packs a block for every class with taps, also for classes with no pixels (H or W == 1):
+      // step past it before skipping the class, or the next class would run on this one's weights
+      const __nv_bfloat16* wcls = wd;
+      wd += (size_t)cp->Cin * nt * Coutp;
       const int subH = (cp->H - ph + s - 1) / s, subW = (cp->W - pw + s - 1) / s;
       if (subH <= 0 || subW <= 0) continue;
       ETB_CHECK_ARG(nt > 0);   // k >= stride for every conv of the trunk, so every parity class is reached
       GemmGeom g;
       g.a_ptr = dy_bf16; g.aN = cp->N; g.aH = Ho; g.aW = Wo; g.aC = cp->Cout; g.a_cstride = cp->x_cstride;
-      g.b_ptr = wd; g.b_rows = cp->Cin;
+      g.b_ptr = wcls; g.b_rows = cp->Cin;
       g.tile_H = subH; g.tile_W = subW;
       g.flat = (k == 1 && s == 1 && pad == 0);
       ka.ntaps = nt;
@@ -618,7 +622,6 @@ extern "C" int etb_conv_dgrad(const void* dy_bf16, const void* wd_bf16, void* dx
       ka.y = (__nv_bfloat16*)dx_bf16;
       int rc = launch_gemm(g, ka, (cudaStream_t)stream);
       if (rc != ETB_OK) return rc;
-      wd += (size_t)cp->Cin * nt * Coutp;
     }
   return ETB_OK;
 }
@@ -801,6 +804,13 @@ static void pick_tile16(int Wo, int Ho, int maxrows, int* TW, int* TH) {
       const double eff = (double)Wo * Ho / ((double)tiles * tw * th) * (tw * th >= maxrows / 2 ? 1.0 : 0.8);
       if (eff > best + 1e-9) { best = eff; *TW = tw; *TH = th; }
     }
+  if (best >= 0.0) return;
+  // maps of at most 3 pixels (1x1, 1x2, 1x3, 2x1, 3x1): no box stays within twice the map, so take the smallest box that
+  // covers it in one tile.  Its extra rows are out of the image for both operands (zero-filled): wasted, never wrong.
+  int best_rows = maxrows + 1;
+  for (int tw = Wo; tw <= maxrows; ++tw)
+    for (int th = Ho; th * tw <= maxrows; ++th)
+      if ((tw * th) % 16 == 0 && tw * th < best_rows) { best_rows = tw * th; *TW = tw; *TH = th; }
 }
 
 // ---- second stage of the split-K: sum the slices, emit the parameter layout, optionally accumulate ----
@@ -909,16 +919,20 @@ __global__ void __launch_bounds__(256) wgrad_reduce_taps_kernel(const float* __r
   for (int i = threadIdx.x; i < CW * kk; i += 256) o[i] = (flags & 2) ? o[i] + sm[i] : sm[i];
 }
 
-static void wgrad_plan(const EtbConvParams* cp, int* BN_, int* TW, int* TH, int* tiles_w, int* tiles_h, int* nimg, int* out_tiles, int* splitk) {
+static int wgrad_plan(const EtbConvParams* cp, int* BN_, int* TW, int* TH, int* tiles_w, int* tiles_h, int* nimg, int* out_tiles, int* splitk) {
   const int Ho = (cp->H + 2 * cp->pad - cp->kh) / cp->stride + 1;
   const int Wo = (cp->W + 2 * cp->pad - cp->kw) / cp->stride + 1;
+  ETB_CHECK_ARG(Ho > 0 && Wo > 0);
   const int BN = cp->Cin >= 128 ? 128 : 64;
   const bool flat = (cp->kh == 1 && cp->kw == 1 && cp->stride == 1 && cp->pad == 0);
+  *TW = *TH = 0;
   if (flat) {
     const long npix = (long)cp->N * cp->H * cp->W;
     *TW = WGRAD_KP; *TH = 1; *tiles_w = (int)((npix + WGRAD_KP - 1) / WGRAD_KP); *tiles_h = 1; *nimg = 1;
   } else {
     pick_tile16(Wo, Ho, WGRAD_KP, TW, TH);
+    // a K tile is a positive whole number of K=16 steps and fits the stage: anything else is a hole in the plan
+    ETB_CHECK_ARG(*TW > 0 && *TH > 0 && (*TW * *TH) % 16 == 0 && *TW * *TH <= WGRAD_KP);
     *tiles_w = (Wo + *TW - 1) / *TW; *tiles_h = (Ho + *TH - 1) / *TH; *nimg = cp->N;
   }
   const int ntaps = cp->kh * cp->kw;
@@ -942,12 +956,13 @@ static void wgrad_plan(const EtbConvParams* cp, int* BN_, int* TW, int* TH, int*
     if (cost < best) { best = cost; sk = c; }
   }
   *splitk = sk; *BN_ = BN;
+  return ETB_OK;
 }
 
 extern "C" size_t etb_conv_wgrad_workspace_bytes(const EtbConvParams* cp) {
-  if (!cp || cp->Cin <= 0 || cp->Cout <= 0) return 0;
+  if (!cp || cp->N <= 0 || cp->H <= 0 || cp->W <= 0 || cp->Cin <= 0 || cp->Cout <= 0 || cp->stride <= 0) return 0;
   int BN, TW, TH, tw, th, ni, ot, sk;
-  wgrad_plan(cp, &BN, &TW, &TH, &tw, &th, &ni, &ot, &sk);
+  if (wgrad_plan(cp, &BN, &TW, &TH, &tw, &th, &ni, &ot, &sk) != ETB_OK) return 0;
   return (size_t)sk * cp->Cout * cp->kh * cp->kw * cp->Cin * sizeof(float);
 }
 
@@ -971,7 +986,8 @@ extern "C" int etb_conv_wgrad(const void* x_bf16, const void* dy_bf16, float* dw
   WgradArgs wa;
   memset(&wa, 0, sizeof(wa));
   int BN, out_tiles, splitk;
-  wgrad_plan(cp, &BN, &wa.TW, &wa.TH, &wa.tiles_w, &wa.tiles_h, &wa.nimg, &out_tiles, &splitk);
+  const int prc = wgrad_plan(cp, &BN, &wa.TW, &wa.TH, &wa.tiles_w, &wa.tiles_h, &wa.nimg, &out_tiles, &splitk);
+  if (prc != ETB_OK) return prc;
   wa.kpix = wa.TW * wa.TH;
   wa.ntaps = cp->kh * cp->kw;
   wa.kw = cp->kw; wa.pad = cp->pad;
