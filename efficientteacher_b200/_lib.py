@@ -151,11 +151,6 @@ _SIGS = {
     "etb_domain_focal_bwd": (C.c_int, [C.POINTER(EtbFocalParams), vp, vp]),
     "etb_val_process_batch": (C.c_int, [vp, vp, C.c_int32, C.c_int32, C.c_int32, vp, C.c_int32, vp, C.c_int32, vp, vp, vp]),
     "etb_nms_boxes": (C.c_int, [vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_float, vp, vp, vp]),
-    "etb_bn_fused_rows": (C.c_int32, [C.c_int64, C.c_int32, C.c_int32]),
-    "etb_bn_fwd_fused": (C.c_int, [vp, C.c_int64, C.c_int32, C.c_int32, vp, vp, C.c_float, C.c_float, vp, vp, vp, vp, C.c_int32, vp, C.c_int32,
-                                  C.c_int32, vp, C.c_int32, vp, vp]),
-    "etb_bn_bwd_fused": (C.c_int, [vp, vp, vp, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp, vp, vp, vp, C.c_int32, vp,
-                                  C.c_int32, vp, vp]),
     "etb_stem_im2col_into": (C.c_int, [vp, C.c_int32, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_float, vp]),
     "etb_tal_workspace_bytes": (C.c_size_t, [C.c_int32, C.c_int32, C.c_int32]),
     "etb_tal_assign": (C.c_int, [vp, vp, vp, vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_float, C.c_float,

@@ -1,6 +1,5 @@
 """Thin Python wrappers over the wgmma convolution and the trunk layout kernels (NHWC bf16 tensors)."""
 import ctypes as C
-import os
 
 import torch
 
@@ -168,20 +167,6 @@ def conv_wgrad(x, dy, Cin, Cout, k, stride, pad, x_coffset=0, dy_coffset=0, stem
 
 
 # ---- training-mode BatchNorm + activation around the convs (csrc/bn.cu) ----
-# ETB_BN_FUSED=1: one cooperative launch per layer and direction (csrc/bn.cu bn_*_fused_kernel) instead of three kernels.
-# Opt-in: it removes 400 launches per step and its kernels are faster in isolation, but a cooperative grid needs the whole
-# GPU to itself, so it serialises against the weight-gradient side stream (slower in the step).
-BN_FUSED = os.environ.get("ETB_BN_FUSED", "0") == "1"
-_bn_barriers = {}
-
-
-def _bn_barrier(device):
-    """the 8-byte grid-barrier state of the fused BN kernels: one per (device, stream), zeroed once"""
-    key = (device.index if device.index is not None else torch.cuda.current_device(), torch.cuda.current_stream(device).cuda_stream)
-    b = _bn_barriers.get(key)
-    if b is None:
-        b = _bn_barriers[key] = torch.zeros(2, dtype=torch.int32, device=device)
-    return b
 
 
 def bn_forward(y, C_, gamma, beta, running_mean, running_var, eps, momentum, act, y_cstride=None, out=None, out_cstride=None,
@@ -194,18 +179,6 @@ def bn_forward(y, C_, gamma, beta, running_mean, running_var, eps, momentum, act
         cs = y_cstride
     M = N * H * W
     lib = _lib.lib()
-    if BN_FUSED:
-        rows = int(lib.etb_bn_fused_rows(M, C_, 0))
-        partials = torch.empty((rows, 2, C_), dtype=torch.float32, device=y.device)
-        stats = torch.empty((4, C_), dtype=torch.float32, device=y.device)
-        if out is None:
-            out = nhwc_empty(N, H, W, C_, y.device)
-        ocs = out.shape[3] if out_cstride is None else out_cstride
-        _lib.check(lib.etb_bn_fwd_fused(_lib.ptr(y), M, C_, cs, _lib.ptr(gamma), _lib.ptr(beta), float(eps), float(momentum),
-                                        _lib.ptr(running_mean), _lib.ptr(running_var), _lib.ptr(stats), None if res is None else _lib.ptr(res),
-                                        0 if res is None else (res.shape[3] if res_cstride is None else res_cstride), _lib.ptr(out), ocs,
-                                        ACT[act], _lib.ptr(partials), rows, _lib.ptr(_bn_barrier(y.device)), _lib.stream_ptr()), "etb_bn_fwd_fused")
-        return out, stats
     rows = int(lib.etb_bn_partial_rows(M, C_, 0))
     partials = torch.empty((rows, 2, C_), dtype=torch.float32, device=y.device)
     _lib.check(lib.etb_bn_stats(_lib.ptr(y), M, C_, cs, _lib.ptr(partials), rows, _lib.stream_ptr()), "etb_bn_stats")
@@ -232,19 +205,6 @@ def bn_backward(da, y, C_, stats, act, da_cstride=None, y_cstride=None, out=None
     dacs = da.shape[3] if da_cstride is None else da_cstride
     M = N * H * W
     lib = _lib.lib()
-    if BN_FUSED:
-        rows = int(lib.etb_bn_fused_rows(M, C_, 1))
-        partials = torch.empty((rows, 2, C_), dtype=torch.float32, device=y.device)
-        sums = torch.empty(2 * C_, dtype=torch.float32, device=y.device)
-        acc = dgamma_into is not None and dbeta_into is not None
-        dgb = None if acc else torch.empty((2, C_), dtype=torch.float32, device=y.device)
-        if out is None:
-            out = nhwc_empty(N, H, W, C_, y.device)
-        _lib.check(lib.etb_bn_bwd_fused(_lib.ptr(da), _lib.ptr(y), _lib.ptr(stats), M, C_, dacs, ycs, out.shape[3], ACT[act], _lib.ptr(out),
-                                        _lib.ptr(sums), _lib.ptr(dgamma_into if acc else dgb[0]), _lib.ptr(dbeta_into if acc else dgb[1]),
-                                        1 if acc else 0, _lib.ptr(partials), rows, _lib.ptr(_bn_barrier(y.device)), _lib.stream_ptr()),
-                   "etb_bn_bwd_fused")
-        return (out, None, None) if acc else (out, dgb[0], dgb[1])
     rows = int(lib.etb_bn_partial_rows(M, C_, 1))
     partials = torch.empty((rows, 2, C_), dtype=torch.float32, device=y.device)
     _lib.check(lib.etb_bn_act_bwd_reduce(_lib.ptr(da), _lib.ptr(y), _lib.ptr(stats[0]), _lib.ptr(stats[1]), _lib.ptr(stats[2]),

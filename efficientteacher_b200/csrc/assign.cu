@@ -18,7 +18,6 @@ __global__ void __launch_bounds__(1024) select_targets_kernel(const double* __re
                                                               int32_t n_host, int32_t cap, const double* __restrict__ thr_high,
                                                               const double* __restrict__ thr_low, int32_t nc, int32_t with_obj,
                                                               float* __restrict__ out, int32_t* __restrict__ out_cnt) {
-  ETB_PDL_PROLOGUE();
   __shared__ int sscan[33];
   int n = n_dev ? *n_dev : n_host;
   if (n > cap) n = cap;
@@ -90,7 +89,6 @@ struct AssignArgs {
 };
 
 __global__ void __launch_bounds__(1024) build_targets_kernel(const AssignArgs A) {
-  ETB_PDL_PROLOGUE();
   __shared__ int sscan[33];
   const int l = blockIdx.x;
   const int nx = A.lv.nx[l], ny = A.lv.ny[l];

@@ -131,7 +131,6 @@ __device__ __forceinline__ void reduce_partials(const float* __restrict__ partia
 
 // ---- forward statistics: sums[0][c] = sum y, sums[1][c] = sum y^2 ----
 __global__ void __launch_bounds__(BN_THREADS) bn_stats_kernel(const __nv_bfloat16* __restrict__ y, int M, int C, int cs, float* __restrict__ sums) {
-  ETB_PDL_PROLOGUE();
   channel_reduce<2, 8, uint4>(M, C, [&](int r, int g) { return ldg_stream(y + (size_t)r * cs + g * 8); },
                               [&](const uint4 v, float (*acc)[8]) {
     float f[8];
@@ -149,7 +148,6 @@ __global__ void __launch_bounds__(BNR_CH * BNR_GR) bn_finalize_kernel(const floa
                                                                        float* __restrict__ running_var, float* __restrict__ scale,
                                                                        float* __restrict__ shift, float* __restrict__ mean_out,
                                                                        float* __restrict__ invstd_out) {
-  ETB_PDL_PROLOGUE();
   const int c = blockIdx.x * BNR_CH + threadIdx.x;
   float sum = 0.f, sumsq = 0.f;
   reduce_partials<BNR_CH, BNR_GR>(partials, nb, C, c, &sum, &sumsq);
@@ -194,7 +192,6 @@ __device__ __forceinline__ float dsilu_f(float z) {
 __global__ void __launch_bounds__(BN_THREADS) bn_act_apply_kernel(const __nv_bfloat16* __restrict__ y, const float* __restrict__ scale,
                                                                   const float* __restrict__ shift, __nv_bfloat16* __restrict__ out, long M, int C,
                                                                   int ycs, int ocs, int act, const __nv_bfloat16* __restrict__ res, int rcs) {
-  ETB_PDL_PROLOGUE();
   const int G = C >> 3;
   const int lg = 31 - __clz(G);            // G is a power of two (checked on the host): no 64-bit divisions
   const long total = M * G;
@@ -250,7 +247,6 @@ __global__ void __launch_bounds__(BN_THREADS) bn_act_bwd_reduce_kernel(const __n
                                                                        const float* __restrict__ scale, const float* __restrict__ shift,
                                                                        const float* __restrict__ mean, const float* __restrict__ invstd, int M,
                                                                        int C, int dacs, int ycs, int act, float* __restrict__ sums) {
-  ETB_PDL_PROLOGUE();
   // per-thread channel group is fixed: hoist its parameters out of the row loop
   float sc[8], sh[8], mu[8], is[8];
   {
@@ -283,7 +279,6 @@ __global__ void __launch_bounds__(BN_THREADS) bn_act_bwd_reduce_kernel(const __n
 template <int BNR_CH, int BNR_GR>
 __global__ void __launch_bounds__(BNR_CH * BNR_GR) bn_bwd_finalize_kernel(const float* __restrict__ partials, int nb, int C, float* __restrict__ sums,
                                                                            float* __restrict__ dgamma, float* __restrict__ dbeta, int accumulate) {
-  ETB_PDL_PROLOGUE();
   const int c = blockIdx.x * BNR_CH + threadIdx.x;
   float s0 = 0.f, s1 = 0.f;
   reduce_partials<BNR_CH, BNR_GR>(partials, nb, C, c, &s0, &s1);
@@ -307,7 +302,6 @@ __global__ void __launch_bounds__(BN_THREADS, 2) bn_act_bwd_apply_kernel(const _
                                                                       const float* __restrict__ mean, const float* __restrict__ invstd,
                                                                       const float* __restrict__ sums, long M, int C, int dacs, int ycs, int ocs,
                                                                       int act, __nv_bfloat16* __restrict__ dy) {
-  ETB_PDL_PROLOGUE();
   const int G = C >> 3;
   const int lg = 31 - __clz(G);
   const long total = M * G;
@@ -476,333 +470,4 @@ extern "C" int etb_bn_act_bwd_apply(const void* da_bf16, const void* y_bf16, con
       act, (__nv_bfloat16*)dy_bf16);
   ETB_CHECK_LAUNCH();
   return ETB_OK;
-}
-
-// =====================================================================================================================
-// Fused (cooperative) variants: statistics -> finalize -> apply in ONE launch, forward and backward.
-// The three-kernel sequences above cost ~35 us (forward) / ~85 us (backward) per layer inside the step even when the layer's
-// activation is a few MB and L2-resident -- 60 of YOLOv5l's 101 BN layers: the time is launch latency, grid ramp-up and the
-// dependent-kernel gaps, not bandwidth.  Here one co-resident grid (cudaLaunchAttributeCooperative, sized to one wave by the
-// occupancy query) runs all three phases separated by two grid barriers:
-//   phase 1  every block reduces its rows (same channel_reduce as above) -> partials[block][2][C]
-//   barrier
-//   phase 2  block b finalizes channels b, b+grid, ...: 256 threads sum the grid's partial rows in a fixed order (thread t:
-//            rows t, t+256, ...; then a fixed-shape tree) -> scale/shift/mean/invstd + running statistics (forward) or the
-//            two backward sums + dgamma/dbeta accumulation (backward): still deterministic, no atomics on data
-//   barrier
-//   phase 3  the elementwise pass, parameters read with ld.global.cg (written by other SMs in phase 2)
-// HBM traffic is unchanged (the second read of y / da hits L2 for the small layers exactly as before); what disappears is
-// 2 launches + 2 kernel boundaries per layer and direction (~400 of the step's ~1270 launches).
-// The barrier is a count + generation pair in a caller-owned 8-byte buffer (zero-initialised once, self-resetting, one per
-// stream); every spin is bounded (trap after ~2 s) so a broken launch fails loudly instead of hanging the box.
-// =====================================================================================================================
-__device__ __forceinline__ void bn_grid_barrier(unsigned* bar) {
-  __syncthreads();
-  if (threadIdx.x == 0 && threadIdx.y == 0) {
-    volatile unsigned* gen = bar + 1;
-    const unsigned my_gen = *gen;
-    __threadfence();
-    const unsigned arrived = atomicAdd(bar, 1u);
-    if (arrived == gridDim.x - 1) {
-      bar[0] = 0u;
-      __threadfence();
-      atomicAdd(bar + 1, 1u);
-    } else {
-      const long long t0 = clock64();
-      while (*gen == my_gen) {
-        if (clock64() - t0 > 4000000000ll) {
-          printf("etb bn: grid barrier timeout (block %d of %d)\n", blockIdx.x, gridDim.x);
-          __trap();
-        }
-      }
-    }
-    __threadfence();
-  }
-  __syncthreads();
-}
-
-__device__ __forceinline__ float bn_block_sum(float v, float* red /*[8]*/) {   // 256 threads, fixed-shape tree
-  v = warp_sum(v);
-  __syncthreads();
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-  __syncthreads();
-  float s = 0.f;
-#pragma unroll
-  for (int w = 0; w < BN_THREADS / 32; ++w) s += red[w];
-  return s;
-}
-__device__ __forceinline__ void ldcg8(const float* p, float* f) {   // parameters produced by other SMs during this kernel
-  const float4 a = __ldcg(reinterpret_cast<const float4*>(p)), b = __ldcg(reinterpret_cast<const float4*>(p) + 1);
-  f[0] = a.x; f[1] = a.y; f[2] = a.z; f[3] = a.w; f[4] = b.x; f[5] = b.y; f[6] = b.z; f[7] = b.w;
-}
-
-struct BnFusedFwd {
-  const __nv_bfloat16* y; long M; int C, ycs;
-  float* partials;                       // [grid][2][C]
-  const float *gamma, *beta; float eps, momentum;
-  float *running_mean, *running_var;
-  float* stats;                          // [4][C]: scale, shift, mean, invstd
-  __nv_bfloat16* out; int ocs, act;
-  const __nv_bfloat16* res; int rcs;
-  unsigned* bar;
-};
-
-__global__ void __launch_bounds__(BN_THREADS) bn_fwd_fused_kernel(const BnFusedFwd a) {
-  ETB_PDL_PROLOGUE();
-  __shared__ float red[8];
-  const int C = a.C;
-  // ---- phase 1: per-block partial sums
-  channel_reduce<2, 8, uint4>((int)a.M, C, [&](int r, int g) { return ldg_stream(a.y + (size_t)r * a.ycs + g * 8); },
-                              [&](const uint4 v, float (*acc)[8]) {
-    float f[8];
-    unpack8(v, f);
-#pragma unroll
-    for (int j = 0; j < 8; ++j) { acc[0][j] += f[j]; acc[1][j] = fmaf(f[j], f[j], acc[1][j]); }
-  }, a.partials);
-  bn_grid_barrier(a.bar);
-  // ---- phase 2: finalize (channels blockIdx.x, +gridDim.x, ...)
-  const int nb = (int)gridDim.x;
-  for (int c = blockIdx.x; c < C; c += nb) {
-    float s0 = 0.f, s1 = 0.f;
-    for (int r = threadIdx.x; r < nb; r += BN_THREADS) {
-      s0 += __ldcg(a.partials + (size_t)r * 2 * C + c);
-      s1 += __ldcg(a.partials + (size_t)r * 2 * C + C + c);
-    }
-    s0 = bn_block_sum(s0, red);
-    s1 = bn_block_sum(s1, red);
-    if (threadIdx.x == 0) {
-      const float inv = 1.0f / (float)a.M;
-      const float mean = s0 * inv;
-      float var = fmaf(-mean, mean, s1 * inv);
-      var = fmaxf(var, 0.0f);
-      const float invstd = rsqrtf(var + a.eps);
-      const float sc = a.gamma[c] * invstd;
-      a.stats[c] = sc;
-      a.stats[C + c] = fmaf(-mean, sc, a.beta[c]);
-      a.stats[2 * C + c] = mean;
-      a.stats[3 * C + c] = invstd;
-      if (a.running_mean) {
-        const float unbiased = a.M > 1 ? var * ((float)a.M / (float)(a.M - 1)) : var;
-        a.running_mean[c] = fmaf(a.momentum, mean - a.running_mean[c], a.running_mean[c]);
-        a.running_var[c] = fmaf(a.momentum, unbiased - a.running_var[c], a.running_var[c]);
-      }
-    }
-  }
-  bn_grid_barrier(a.bar);
-  // ---- phase 3: a = act(y*scale + shift) (+ res)
-  const int G = C >> 3;
-  const int lg = 31 - __clz(G);
-  const long total = a.M * G;
-  const long stride = (long)gridDim.x * blockDim.x;
-  long e = (long)blockIdx.x * blockDim.x + threadIdx.x;
-  const int g = (int)(e & (G - 1));
-  float sc[8], sh[8];
-  ldcg8(a.stats + g * 8, sc); ldcg8(a.stats + C + g * 8, sh);
-  const __nv_bfloat16* y = a.y + g * 8;
-  __nv_bfloat16* out = a.out + g * 8;
-  const __nv_bfloat16* res = a.res ? a.res + g * 8 : nullptr;
-  const int act = a.act;
-  auto body = [&](float* f, long r) {
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const float z = fmaf(f[j], sc[j], sh[j]);
-      f[j] = act == 1 ? silu_f(z) : (act == 2 ? fmaxf(z, 0.f) : z);
-    }
-    if (res) {
-      float q[8];
-      load8(res + r * a.rcs, q);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) f[j] += q[j];
-    }
-  };
-  for (; e + stride < total; e += 2 * stride) {
-    const long r0 = e >> lg, r1 = (e + stride) >> lg;
-    float f0[8], f1[8];
-    load8(y + r0 * a.ycs, f0);
-    load8(y + r1 * a.ycs, f1);
-    body(f0, r0);
-    body(f1, r1);
-    store8(out + r0 * a.ocs, f0);
-    store8(out + r1 * a.ocs, f1);
-  }
-  if (e < total) {
-    const long r0 = e >> lg;
-    float f0[8];
-    load8(y + r0 * a.ycs, f0);
-    body(f0, r0);
-    store8(out + r0 * a.ocs, f0);
-  }
-}
-
-struct BnFusedBwd {
-  const __nv_bfloat16 *da, *y; long M; int C, dacs, ycs, ocs, act;
-  const float* stats;                    // [4][C] from the forward
-  float* partials;                       // [grid][2][C]
-  float* sums;                           // [2][C]
-  float *dgamma, *dbeta; int accumulate;
-  __nv_bfloat16* dy;
-  unsigned* bar;
-};
-
-__global__ void __launch_bounds__(BN_THREADS, 3) bn_bwd_fused_kernel(const BnFusedBwd a) {
-  ETB_PDL_PROLOGUE();
-  __shared__ float red[8];
-  const int C = a.C;
-  const float *scale = a.stats, *shift = a.stats + C, *mean = a.stats + 2 * C, *invstd = a.stats + 3 * C;
-  {
-    // ---- phase 1: sums of dz and dz*xhat per block
-    float sc[8], sh[8], mu[8], is[8];
-    const int g0 = threadIdx.x % (C >> 3);
-    ldf8(scale + g0 * 8, sc); ldf8(shift + g0 * 8, sh); ldf8(mean + g0 * 8, mu); ldf8(invstd + g0 * 8, is);
-#pragma unroll
-    for (int j = 0; j < 8; ++j) mu[j] = -mu[j] * is[j];
-    const int act = a.act;
-    channel_reduce<2, 4, Vec2>((int)a.M, C, [&](int r, int g) {
-      Vec2 v;
-      v.a = ldg_stream(a.y + (size_t)r * a.ycs + g * 8);
-      v.b = ldg_stream(a.da + (size_t)r * a.dacs + g * 8);
-      return v;
-    }, [&](const Vec2 v, float (*acc)[8]) {
-      float fy[8], fd[8];
-      unpack8(v.a, fy);
-      unpack8(v.b, fd);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const float z = fmaf(fy[j], sc[j], sh[j]);
-        const float dz = fd[j] * (act == 1 ? dsilu_f(z) : (act == 2 ? (z > 0.f ? 1.f : 0.f) : 1.f));
-        const float xh = fmaf(fy[j], is[j], mu[j]);
-        acc[0][j] += dz;
-        acc[1][j] = fmaf(dz, xh, acc[1][j]);
-      }
-    }, a.partials);
-  }
-  bn_grid_barrier(a.bar);
-  // ---- phase 2: totals, dbeta / dgamma
-  const int nb = (int)gridDim.x;
-  for (int c = blockIdx.x; c < C; c += nb) {
-    float s0 = 0.f, s1 = 0.f;
-    for (int r = threadIdx.x; r < nb; r += BN_THREADS) {
-      s0 += __ldcg(a.partials + (size_t)r * 2 * C + c);
-      s1 += __ldcg(a.partials + (size_t)r * 2 * C + C + c);
-    }
-    s0 = bn_block_sum(s0, red);
-    s1 = bn_block_sum(s1, red);
-    if (threadIdx.x == 0) {
-      a.sums[c] = s0;
-      a.sums[C + c] = s1;
-      if (a.accumulate) { a.dbeta[c] += s0; a.dgamma[c] += s1; }
-      else { a.dbeta[c] = s0; a.dgamma[c] = s1; }
-    }
-  }
-  bn_grid_barrier(a.bar);
-  // ---- phase 3: dy = gamma*invstd * (dz - sum_dz/M - xhat*sum_dz_xhat/M)
-  const int G = C >> 3;
-  const int lg = 31 - __clz(G);
-  const long total = a.M * G;
-  const float invM = 1.0f / (float)a.M;
-  const long stride = (long)gridDim.x * blockDim.x;
-  long e = (long)blockIdx.x * blockDim.x + threadIdx.x;
-  const int g = (int)(e & (G - 1));
-  float sc[8], sh[8], P[8], Q[8];
-  {
-    float a1[8], mu[8], k0[8], k1[8];
-    ldf8(scale + g * 8, sc); ldf8(shift + g * 8, sh); ldf8(invstd + g * 8, a1); ldf8(mean + g * 8, mu);
-    ldcg8(a.sums + g * 8, k0); ldcg8(a.sums + C + g * 8, k1);
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const float k1m = k1[j] * invM * a1[j];
-      P[j] = -sc[j] * k1m;
-      Q[j] = -sc[j] * fmaf(-mu[j], k1m, k0[j] * invM);
-    }
-  }
-  const __nv_bfloat16* y = a.y + g * 8;
-  const __nv_bfloat16* da = a.da + g * 8;
-  __nv_bfloat16* dy = a.dy + g * 8;
-  const int act = a.act;
-  auto body = [&](const float* fy, float* fd) {
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const float z = fmaf(fy[j], sc[j], sh[j]);
-      const float dz = fd[j] * (act == 1 ? dsilu_f(z) : (act == 2 ? (z > 0.f ? 1.f : 0.f) : 1.f));
-      fd[j] = fmaf(sc[j], dz, fmaf(fy[j], P[j], Q[j]));
-    }
-  };
-  for (; e + stride < total; e += 2 * stride) {
-    const long r0 = e >> lg, r1 = (e + stride) >> lg;
-    float y0[8], d0[8], y1[8], d1[8];
-    load8(y + r0 * a.ycs, y0);
-    load8(da + r0 * a.dacs, d0);
-    load8(y + r1 * a.ycs, y1);
-    load8(da + r1 * a.dacs, d1);
-    body(y0, d0);
-    body(y1, d1);
-    store8(dy + r0 * a.ocs, d0);
-    store8(dy + r1 * a.ocs, d1);
-  }
-  if (e < total) {
-    const long r0 = e >> lg;
-    float y0[8], d0[8];
-    load8(y + r0 * a.ycs, y0);
-    load8(da + r0 * a.dacs, d0);
-    body(y0, d0);
-    store8(dy + r0 * a.ocs, d0);
-  }
-}
-
-template <typename A>
-static inline int bn_launch_coop(void (*kernel)(const A), unsigned grid, const A& args, cudaStream_t st) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(grid);
-  cfg.blockDim = dim3(BN_THREADS);
-  cfg.dynamicSmemBytes = 0;
-  cfg.stream = st;
-  cudaLaunchAttribute at[2];
-  at[0].id = cudaLaunchAttributeCooperative;
-  at[0].val.cooperative = 1;
-  at[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  at[1].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = at;
-  cfg.numAttrs = etb_pdl_enabled() ? 2 : 1;
-  ETB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kernel, args));
-  etb_count_launch();
-  return ETB_OK;
-}
-
-// grid of the fused kernels = rows of their partial buffer ([rows][2][C] floats); which = 0 forward, 1 backward
-extern "C" int32_t etb_bn_fused_rows(int64_t M, int32_t C, int32_t which) {
-  if (M <= 0 || !bn_c_ok(C)) return 0;
-  const long wave = which ? BN_WAVE(bn_bwd_fused_kernel) : BN_WAVE(bn_fwd_fused_kernel);
-  long need = (M * (C / 8) + BN_THREADS - 1) / BN_THREADS;       // one 16 B vector per thread in the elementwise phase
-  if (need > wave) need = wave;
-  return (int32_t)(need < 1 ? 1 : need);
-}
-
-// act(BatchNorm_train(y)) (+ res) in one cooperative launch: statistics, finalize (incl. the running-statistics update) and
-// apply.  stats: [4][C] floats (scale, shift, mean, invstd) for the backward.  partials: [etb_bn_fused_rows(M,C,0)][2][C]
-// floats of scratch.  barrier: 2 x uint32, zeroed once by the caller, owned by one stream.
-extern "C" int etb_bn_fwd_fused(const void* y_bf16, int64_t M, int32_t C, int32_t y_cstride, const float* gamma, const float* beta, float eps,
-                                float momentum, float* running_mean, float* running_var, float* stats, const void* res_bf16, int32_t res_cstride,
-                                void* out_bf16, int32_t out_cstride, int32_t act, float* partials, int32_t rows, uint32_t* barrier, void* stream) {
-  ETB_CHECK_ARG(y_bf16 && gamma && beta && stats && out_bf16 && partials && barrier && M > 0 && M < (1ll << 31) && bn_c_ok(C));
-  ETB_CHECK_ARG(y_cstride % 8 == 0 && y_cstride >= C && out_cstride % 8 == 0 && rows == etb_bn_fused_rows(M, C, 0));
-  ETB_CHECK_ARG(!res_bf16 || (res_cstride % 8 == 0 && res_cstride >= C));
-  BnFusedFwd a;
-  a.y = (const __nv_bfloat16*)y_bf16; a.M = (long)M; a.C = C; a.ycs = y_cstride; a.partials = partials; a.gamma = gamma; a.beta = beta;
-  a.eps = eps; a.momentum = momentum; a.running_mean = running_mean; a.running_var = running_var; a.stats = stats;
-  a.out = (__nv_bfloat16*)out_bf16; a.ocs = out_cstride; a.act = act; a.res = (const __nv_bfloat16*)res_bf16; a.rcs = res_cstride; a.bar = barrier;
-  return bn_launch_coop(bn_fwd_fused_kernel, (unsigned)rows, a, (cudaStream_t)stream);
-}
-
-// backward of the above in one cooperative launch: dy (raw conv output gradient) + dgamma / dbeta (written, or added in place
-// when accumulate != 0: the gradient-arena slices).  sums: [2][C] floats of scratch.
-extern "C" int etb_bn_bwd_fused(const void* da_bf16, const void* y_bf16, const float* stats, int64_t M, int32_t C, int32_t da_cstride,
-                                int32_t y_cstride, int32_t dy_cstride, int32_t act, void* dy_bf16, float* sums, float* dgamma, float* dbeta,
-                                int32_t accumulate, float* partials, int32_t rows, uint32_t* barrier, void* stream) {
-  ETB_CHECK_ARG(da_bf16 && y_bf16 && stats && dy_bf16 && sums && dgamma && dbeta && partials && barrier && M > 0 && M < (1ll << 31) && bn_c_ok(C));
-  ETB_CHECK_ARG(da_cstride % 8 == 0 && y_cstride % 8 == 0 && dy_cstride % 8 == 0 && rows == etb_bn_fused_rows(M, C, 1));
-  BnFusedBwd a;
-  a.da = (const __nv_bfloat16*)da_bf16; a.y = (const __nv_bfloat16*)y_bf16; a.M = (long)M; a.C = C; a.dacs = da_cstride; a.ycs = y_cstride;
-  a.ocs = dy_cstride; a.act = act; a.stats = stats; a.partials = partials; a.sums = sums; a.dgamma = dgamma; a.dbeta = dbeta;
-  a.accumulate = accumulate; a.dy = (__nv_bfloat16*)dy_bf16; a.bar = barrier;
-  return bn_launch_coop(bn_bwd_fused_kernel, (unsigned)rows, a, (cudaStream_t)stream);
 }

@@ -39,33 +39,7 @@ void etb_count_launch();   // every ETB_CHECK_LAUNCH() follows exactly one kerne
     }                                                                                    \
   } while (0)
 
-// ---- programmatic dependent launch (PDL) -----------------------------------------------------------------------------
-// Every kernel of the library is launched with cudaLaunchAttributeProgrammaticStreamSerialization and starts with
-// ETB_PDL_PROLOGUE(): `griddepcontrol.wait` (returns when the preceding kernel of the stream has completed and its memory is
-// visible -- so no kernel touches global data before its producer is done) followed by `griddepcontrol.launch_dependents`
-// (the NEXT kernel's CTAs may be scheduled as soon as all CTAs of this one have passed this point or exited).  The next
-// kernel's launch latency, block scheduling and prologue (smem carve-up, mbarrier init, tensor-map
-// prefetch: the conv kernels place the wait after that prologue) thereby overlap this kernel's execution instead of
-// following its tail.  Once the step is replayed as a CUDA graph the graph's kernel-to-kernel latency is already small,
-// so the attribute is only set with ETB_PDL=1 (eager-launch experiments).  A kernel launched without the attribute (ETB_PDL=0, or a neighbour from another library) sees both instructions
-// as no-ops / full stream order, so mixing is safe.  Captured CUDA graphs keep the programmatic edges.
-#define ETB_PDL_WAIT() asm volatile("griddepcontrol.wait;" ::: "memory")
-#define ETB_PDL_TRIGGER() asm volatile("griddepcontrol.launch_dependents;" ::: "memory")
-#define ETB_PDL_PROLOGUE() \
-  do {                     \
-    ETB_PDL_WAIT();        \
-    ETB_PDL_TRIGGER();     \
-  } while (0)
-
-static inline bool etb_pdl_enabled() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("ETB_PDL");
-    v = (e && e[0] == '1') ? 1 : 0;       // opt-in: eager-launch experiments
-  }
-  return v != 0;
-}
-
+// The library's one launch helper: arguments are converted to the kernel's parameter types, as a <<<>>> launch would.
 template <typename... KP, typename... A>
 static inline void etb_launch(void (*kernel)(KP...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, A&&... args) {
   cudaLaunchConfig_t cfg = {};
@@ -73,11 +47,7 @@ static inline void etb_launch(void (*kernel)(KP...), dim3 grid, dim3 block, size
   cfg.blockDim = block;
   cfg.dynamicSmemBytes = smem;
   cfg.stream = st;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  at[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = at;
-  cfg.numAttrs = etb_pdl_enabled() ? 1 : 0;
+  cfg.numAttrs = 0;
   (void)cudaLaunchKernelEx(&cfg, kernel, static_cast<KP>(args)...);    // the caller checks cudaGetLastError() (ETB_CHECK_LAUNCH)
 }
 

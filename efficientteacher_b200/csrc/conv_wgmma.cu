@@ -274,7 +274,6 @@ conv_fwd_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
     fence_barrier_init();
   }
   __syncthreads();
-  ETB_PDL_PROLOGUE();      // everything above (barriers, descriptor prefetch) overlapped the previous kernel's tail
 
   if (wg == 0) {
     if (warp != 0) return;
@@ -552,7 +551,6 @@ extern "C" int64_t etb_dgrad_weight_elems(int32_t Cout, int32_t Cin, int32_t k, 
 
 struct TapTable { signed char v[24]; };
 __global__ void __launch_bounds__(256) pack_weight_dgrad_kernel(const float* __restrict__ w, __nv_bfloat16* __restrict__ o, int Cout, int Coutp, int Cin, int k, int ntaps, TapTable tt) {
-  ETB_PDL_PROLOGUE();
   const int64_t total = (int64_t)Cin * ntaps * Coutp;
   for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (int64_t)gridDim.x * blockDim.x) {
     const int co = (int)(e % Coutp);
@@ -706,7 +704,6 @@ wgrad_kernel(const __grid_constant__ CUtensorMap mapDy, const __grid_constant__ 
     fence_barrier_init();
   }
   __syncthreads();
-  ETB_PDL_PROLOGUE();      // prologue above overlapped the previous kernel's tail; no global data touched before this
   const uint32_t box_bytes = (uint32_t)a.kpix * 128u;   // bytes one TMA box writes (all rows, OOB rows zero-filled)
 
   if (wg == 0) {
@@ -820,7 +817,6 @@ static void pick_tile16(int Wo, int Ho, int maxrows, int* TW, int* TH) {
 template <int SG>
 __global__ void __launch_bounds__(32 * SG) wgrad_reduce_kernel(const float* __restrict__ ws, long slice, int splitk, float* __restrict__ out, int Cout,
                                                                int Cin, int kk, int flags) {
-  ETB_PDL_PROLOGUE();
   __shared__ float4 red[SG][32];
   const long n4 = (long)Cout * kk * Cin / 4;
   const int lane = threadIdx.x, sg = threadIdx.y;
@@ -887,7 +883,6 @@ __global__ void __launch_bounds__(32 * SG) wgrad_reduce_kernel(const float* __re
 // scatter cost 8x sector amplification on both the read-modify-write and the store (60 us per 3x3 layer).
 __global__ void __launch_bounds__(256) wgrad_reduce_taps_kernel(const float* __restrict__ ws, long slice, int splitk, float* __restrict__ out, int Cin,
                                                                 int kk, int flags) {
-  ETB_PDL_PROLOGUE();
   __shared__ float sm[64 * 12];
   const int CW = Cin < 64 ? Cin : 64;            // channels per block (Cin is a multiple of 64, or smaller than 64 and of 8)
   const int L4 = CW >> 2;                        // float4 lanes per tap

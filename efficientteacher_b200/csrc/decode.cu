@@ -15,7 +15,6 @@ struct DecodeArgs {
 };
 
 __global__ void __launch_bounds__(256) detect_decode_kernel(const DecodeArgs A) {
-  ETB_PDL_PROLOGUE();
   const int64_t per_img = (int64_t)A.na * A.ny * A.nx * A.no;
   const int64_t total = per_img * A.B;
   for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (int64_t)gridDim.x * blockDim.x) {

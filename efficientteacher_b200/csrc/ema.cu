@@ -13,7 +13,6 @@ __device__ __forceinline__ float ema1(float v, float m, float d, float omd) {
 // `dev` (optional): {d, 1-d, d2, 1-d2} in device memory -- lets a captured CUDA graph replay with a new decay each step
 __global__ void __launch_bounds__(256) ema_kernel(const EtbEmaChunk* __restrict__ tab, float d, float omd, float d2, float omd2,
                                                   const float* __restrict__ dev) {
-  ETB_PDL_PROLOGUE();
   if (dev) { d = dev[0]; omd = dev[1]; d2 = dev[2]; omd2 = dev[3]; }
   const EtbEmaChunk c = tab[blockIdx.x];
   float* __restrict__ v = c.v;

@@ -31,7 +31,6 @@ __device__ __forceinline__ uint4 g_pack8(const float* f) {
 // ---- max pool 5x5 s1 p2 with argmax (window position (dy+2)*5+(dx+2), first maximum in scan order wins like ATen) ----
 __global__ void __launch_bounds__(256) maxpool5_fwd_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat16* __restrict__ y,
                                                            uint8_t* __restrict__ idx, int N, int H, int W, int C, int xcs, int ycs) {
-  ETB_PDL_PROLOGUE();
   const int cg = C >> 3;
   const int64_t total = (int64_t)N * H * W * cg;
   for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (int64_t)gridDim.x * blockDim.x) {
@@ -70,7 +69,6 @@ __global__ void __launch_bounds__(256) maxpool5_fwd_kernel(const __nv_bfloat16* 
 __global__ void __launch_bounds__(256) maxpool5_bwd_kernel(const __nv_bfloat16* __restrict__ src, const uint8_t* __restrict__ idx,
                                                            const __nv_bfloat16* __restrict__ add, __nv_bfloat16* __restrict__ out, int N, int H,
                                                            int W, int C, int scs, int acs, int ocs) {
-  ETB_PDL_PROLOGUE();
   const int cg = C >> 3;
   const int64_t total = (int64_t)N * H * W * cg;
   for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (int64_t)gridDim.x * blockDim.x) {
@@ -133,7 +131,6 @@ extern "C" int etb_maxpool5_bwd(const void* src_bf16, const uint8_t* idx, const 
 // ---- nearest 2x upsample backward: dx[n,h,w,:] = sum of the 2x2 block of dy (fp32 accumulate) ----
 __global__ void __launch_bounds__(256) upsample2x_bwd_kernel(const __nv_bfloat16* __restrict__ dy, __nv_bfloat16* __restrict__ dx, int N, int H, int W,
                                                              int C, int dycs, int dxcs) {
-  ETB_PDL_PROLOGUE();
   const int cg = C >> 3;
   const int64_t total = (int64_t)N * H * W * cg;
   for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (int64_t)gridDim.x * blockDim.x) {
@@ -167,7 +164,6 @@ extern "C" int etb_upsample2x_bwd(const void* dy_bf16, void* dx_bf16, int32_t N,
 // ---- channel-slice copy: y[m, 0:C] = x[m, 0:C] for M pixels, both sides with a channel stride ----
 __global__ void __launch_bounds__(256) copy_slice_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat16* __restrict__ y, int64_t M, int C, int xcs,
                                                          int ycs) {
-  ETB_PDL_PROLOGUE();
   const int cg = C >> 3;
   const int64_t total = M * cg;
   for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (int64_t)gridDim.x * blockDim.x) {

@@ -97,7 +97,6 @@ __device__ __forceinline__ int64_t cell_index(const EtbLossParams& lp, int l, co
 // -------------------------------------------------------------------------------------------------
 template <bool BWD>
 __global__ void __launch_bounds__(256) loss_rows_kernel(LossPtrs P, EtbLossParams lp, LossSets S, LossWs ws, const float* __restrict__ gscale_dev) {
-  ETB_PDL_PROLOGUE();
   const int lane = threadIdx.x & 31;
   const int nwarps = gridDim.x * (blockDim.x >> 5);
   const int gw = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -181,7 +180,6 @@ __device__ __forceinline__ float cell_tobj(const EtbLossParams& lp, const LossSe
 }
 
 __global__ void __launch_bounds__(256) loss_obj_fwd_kernel(LossPtrs P, EtbLossParams lp, LossSets S, LossWs ws) {
-  ETB_PDL_PROLOGUE();
   __shared__ float ssum[8];
   __shared__ float scnt[8];
   const int l = blockIdx.y;
@@ -208,7 +206,6 @@ __global__ void __launch_bounds__(256) loss_obj_fwd_kernel(LossPtrs P, EtbLossPa
 }
 
 __global__ void loss_finalize_kernel(EtbLossParams lp, LossSets S, LossWs ws, float* __restrict__ out4) {
-  ETB_PDL_PROLOGUE();
   if (threadIdx.x != 0 || blockIdx.x != 0) return;
   const int nc = lp.no - 5;
   // fp32 accumulation in the reference's order: lbox += mean ; lobj += mean*balance ; then the weights
@@ -243,7 +240,6 @@ __global__ void loss_finalize_kernel(EtbLossParams lp, LossSets S, LossWs ws, fl
 // backward of the objectness term + dense zero-fill of every other element: one thread per element,
 // fully coalesced stores.  dL/dx4 = obj_w * B * balance_l / n_valid_l * (sigmoid(x) - tobj) for valid cells.
 __global__ void __launch_bounds__(256) loss_obj_bwd_kernel(LossPtrs P, EtbLossParams lp, LossSets S, LossWs ws, const float* __restrict__ gscale_dev) {
-  ETB_PDL_PROLOGUE();
   const int l = blockIdx.y;
   const int64_t ncell = ws.cell_off[l + 1] - ws.cell_off[l];
   const int64_t nel = ncell * lp.no;
@@ -331,7 +327,6 @@ extern "C" int etb_loss_backward(const float* const* p, float* const* grad_p, co
 
 // ---- standalone bbox_iou (CIoU, xywh, 1-to-1): reference utils/metrics.py:207-249 ----
 __global__ void bbox_ciou_kernel(const float* __restrict__ b1, const float* __restrict__ b2, int n, float* __restrict__ out) {
-  ETB_PDL_PROLOGUE();
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const float4 a = reinterpret_cast<const float4*>(b1)[i], b = reinterpret_cast<const float4*>(b2)[i];

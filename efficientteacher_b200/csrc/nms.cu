@@ -87,7 +87,6 @@ __device__ __forceinline__ bool is_candidate(const float* __restrict__ row, int 
 }
 
 __global__ void __launch_bounds__(256) cand_count_kernel(const float* __restrict__ pred, EtbNmsParams p, NmsWs ws) {
-  ETB_PDL_PROLOGUE();
   const int b = blockIdx.y, chunk = blockIdx.x;
   const float* base = pred + (size_t)b * p.P * p.no;
   int cnt = 0;
@@ -109,7 +108,6 @@ __global__ void __launch_bounds__(256) cand_count_kernel(const float* __restrict
 }
 
 __global__ void __launch_bounds__(256) cand_write_kernel(const float* __restrict__ pred, EtbNmsParams p, NmsWs ws) {
-  ETB_PDL_PROLOGUE();
   __shared__ int sscan[33];
   __shared__ int sbase;
   const int b = blockIdx.y, chunk = blockIdx.x;
@@ -139,7 +137,6 @@ __global__ void __launch_bounds__(256) cand_write_kernel(const float* __restrict
 // One warp per candidate (grid-stride).  Literal order of operations of general.py:936-953:
 //   cls_score = max_c cls_c ; cls_c *= obj ; box = xywh2xyxy ; conf, j = max_c (first maximal index on ties)
 __global__ void __launch_bounds__(256) cand_record_kernel(const float* __restrict__ pred, EtbNmsParams p, NmsWs ws) {
-  ETB_PDL_PROLOGUE();
   const int lane = threadIdx.x & 31;
   const int warps_per_grid = gridDim.x * (blockDim.x >> 5);
   const int gw = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -189,7 +186,6 @@ __global__ void __launch_bounds__(256) cand_record_kernel(const float* __restric
 // ---- C1 --------------------------------------------------------------------------------------------
 // rank_i = #{ j : key_j > key_i  or (key_j == key_i and j < i) }  == position in a stable descending sort.
 __global__ void __launch_bounds__(256) rank_kernel(EtbNmsParams p, NmsWs ws) {
-  ETB_PDL_PROLOGUE();
   __shared__ float sk[256];
   const int b = blockIdx.y;
   const int n1 = ws.n1[b];
@@ -231,7 +227,6 @@ __device__ __forceinline__ bool iou_gt(float ax1, float ay1, float ax2, float ay
 
 __global__ void __launch_bounds__(1024) nms_image_kernel(EtbNmsParams p, NmsWs ws, float* __restrict__ det,
                                                          int32_t* __restrict__ det_cnt, const double* __restrict__ Ms) {
-  ETB_PDL_PROLOGUE();
   __shared__ float kx1[NMS_MAXK], ky1[NMS_MAXK], kx2[NMS_MAXK], ky2[NMS_MAXK], karea[NMS_MAXK];
   __shared__ int kslot[NMS_MAXK];
   __shared__ float tx1[64], ty1[64], tx2[64], ty2[64], tarea[64];
@@ -363,7 +358,6 @@ __global__ void __launch_bounds__(1024) nms_image_kernel(EtbNmsParams p, NmsWs w
 
 // ---- C3 --------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(1024) pl_gather_kernel(EtbNmsParams p, NmsWs ws, double* __restrict__ pl_rows, int32_t* __restrict__ pl_cnt) {
-  ETB_PDL_PROLOGUE();
   int base = 0;
   for (int b = 0; b < p.B; ++b) {
     const int c = ws.pl_seg_cnt[b];
@@ -450,7 +444,6 @@ __device__ __forceinline__ bool ml_row_candidate(const float* __restrict__ row, 
 // level 0: bins = key >> 20 (all valid keys); level 1: (key >> 8) & 0xFFF of keys whose top 12 bits == prefix >> 20;
 // level 2: key & 0xFF of keys whose top 24 bits == prefix >> 8.
 __global__ void __launch_bounds__(256) ml_hist_kernel(const float* __restrict__ pred, EtbNmsParams p, MlWs ws, int level) {
-  ETB_PDL_PROLOGUE();
   __shared__ uint32_t sh[ML_BINS];
   const int b = blockIdx.y, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int nc = p.no - 5;
@@ -480,7 +473,6 @@ __global__ void __launch_bounds__(256) ml_hist_kernel(const float* __restrict__ 
 // One block (256 threads) per image.  Finds, walking the bins from the top, the bin that holds the k_rem-th largest key
 // among the keys that match the digits fixed so far; updates prefix / k_rem / greater; clears the histogram for the next level.
 __global__ void __launch_bounds__(256) ml_select_kernel(EtbNmsParams p, MlWs ws, int level) {
-  ETB_PDL_PROLOGUE();
   __shared__ uint32_t part[256];
   __shared__ int found_bin;
   const int b = blockIdx.x;
@@ -540,7 +532,6 @@ __device__ __forceinline__ void ml_class(uint32_t k, uint32_t T, bool all, int* 
 
 template <bool WRITE>
 __global__ void __launch_bounds__(256) ml_pairs_kernel(const float* __restrict__ pred, EtbNmsParams p, MlWs ws, NmsWs nw, int cap) {
-  ETB_PDL_PROLOGUE();
   __shared__ int row_gt[ML_ROWS], row_eq[ML_ROWS];
   __shared__ int sbase_gt, sbase_eq;
   const int b = blockIdx.y, chunk = blockIdx.x, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;

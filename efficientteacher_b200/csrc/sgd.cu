@@ -8,7 +8,6 @@
 #include "common.cuh"
 
 __global__ void __launch_bounds__(256) sgd_kernel(const EtbSgdChunk* __restrict__ tab, const float* __restrict__ hyper, int zero_grad) {
-  ETB_PDL_PROLOGUE();
   const EtbSgdChunk c = tab[blockIdx.x];
   const float lr = hyper[4 * c.group + 0], mom = hyper[4 * c.group + 1], wd = hyper[4 * c.group + 2];
   float* __restrict__ p = c.p;

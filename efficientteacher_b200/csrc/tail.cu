@@ -16,7 +16,6 @@
 // 170 B runs out; per-channel partial sums of the bias gradient in registers -> partials[(n*chunks + chunk)][C].
 __global__ void __launch_bounds__(128) detect_dy_pack_kernel(const float* __restrict__ g, __nv_bfloat16* __restrict__ dy, float* __restrict__ partials,
                                                              int na, int HW, int no, int Cpad) {
-  ETB_PDL_PROLOGUE();
   const int chunk = blockIdx.x, a = blockIdx.y, n = blockIdx.z;
   const int o = threadIdx.x;
   const int C = na * no;
@@ -40,7 +39,6 @@ __global__ void __launch_bounds__(128) detect_dy_pack_kernel(const float* __rest
 
 // out[c] (+)= sum over rows of partials[row][c]; block (32 channels x 32 row lanes), fixed-shape tree: deterministic
 __global__ void __launch_bounds__(1024) column_sum_kernel(const float* __restrict__ partials, int rows, int C, float* __restrict__ out, int accumulate) {
-  ETB_PDL_PROLOGUE();
   __shared__ float red[32][33];
   const int c = blockIdx.x * 32 + threadIdx.x;
   float a = 0.f;
@@ -92,7 +90,6 @@ __device__ __forceinline__ void bf8_to_f(const uint4 v, float* f) {
 // one warp per pixel row: o[m][j] = sum_c h[m][c] * w2[j][c]
 __global__ void __launch_bounds__(NETD_THREADS) netd_tail_fwd_kernel(const __nv_bfloat16* __restrict__ h, long M, int C, int hcs,
                                                                      const float* __restrict__ w2, float* __restrict__ o) {
-  ETB_PDL_PROLOGUE();
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nw = NETD_THREADS / 32;
   const int G = C >> 3;
   for (long m = (long)blockIdx.x * nw + wid; m < M; m += (long)gridDim.x * nw) {
@@ -117,7 +114,6 @@ __global__ void __launch_bounds__(NETD_THREADS) netd_tail_fwd_kernel(const __nv_
 __global__ void __launch_bounds__(NETD_THREADS) netd_tail_bwd_kernel(const float* __restrict__ dout, const __nv_bfloat16* __restrict__ h, long M, int C,
                                                                      int hcs, const float* __restrict__ w2, __nv_bfloat16* __restrict__ dh,
                                                                      float* __restrict__ partials) {
-  ETB_PDL_PROLOGUE();
   extern __shared__ float sm[];      // [nw][2][C]
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nw = NETD_THREADS / 32;
   const int G = C >> 3;
@@ -216,7 +212,6 @@ __device__ __forceinline__ void focal_terms(float d, float* logp, float* p) {
 }
 
 __global__ void __launch_bounds__(FOCAL_THREADS) focal_fwd_kernel(EtbFocalParams fp, float* __restrict__ partials) {
-  ETB_PDL_PROLOGUE();
   __shared__ float red[FOCAL_THREADS / 32];
   float acc = 0.f;
   for (int l = 0; l < fp.nl; ++l) {
@@ -240,13 +235,11 @@ __global__ void __launch_bounds__(FOCAL_THREADS) focal_fwd_kernel(EtbFocalParams
   }
 }
 __global__ void focal_finalize_kernel(const float* __restrict__ partials, float scale, float* __restrict__ out) {
-  ETB_PDL_PROLOGUE();
   float s = 0.f;
   for (int b = 0; b < FOCAL_BLOCKS; ++b) s += partials[b];      // fixed order
   out[0] = s * scale;
 }
 __global__ void __launch_bounds__(FOCAL_THREADS) focal_bwd_kernel(EtbFocalParams fp, const float* __restrict__ gout, float scale) {
-  ETB_PDL_PROLOGUE();
   const float gs = gout[0] * scale;
   for (int l = 0; l < fp.nl; ++l) {
     const float2* x = reinterpret_cast<const float2*>(fp.x[l]);
@@ -306,7 +299,6 @@ extern "C" int etb_domain_focal_bwd(const EtbFocalParams* fp, const float* gout,
 #define STEM_PITCH 133
 template <typename T>
 __global__ void __launch_bounds__(256) stem_im2col_any_kernel(const T* __restrict__ x, __nv_bfloat16* __restrict__ y, int N, int H, int W, float div) {
-  ETB_PDL_PROLOGUE();
   __shared__ float sm[18 * STEM_PITCH];
   const int Ho = H / 2, Wo = W / 2;
   const int tiles_w = (Wo + STEM_TP - 1) / STEM_TP;

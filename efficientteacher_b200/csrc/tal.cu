@@ -77,7 +77,6 @@ __device__ __forceinline__ int tal_label_index(float lab, int nc) {
 // that lie inside the gt box (mask_topk * mask_in_gts * mask_gt, :97) are counted per anchor.
 // ---------------------------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(TAL_THREADS) tal_topk_kernel(const TalArgs a) {
-  ETB_PDL_PROLOGUE();
   extern __shared__ float smet[];
   __shared__ float s_v[TAL_WARPS];
   __shared__ int s_i[TAL_WARPS];
@@ -158,7 +157,6 @@ __global__ void __launch_bounds__(TAL_THREADS) tal_topk_kernel(const TalArgs a) 
 // background anchors, so their label / box are those of gt 0 (label clamped at 0), exactly as the reference returns them.
 // ---------------------------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) tal_resolve_kernel(const TalArgs a) {
-  ETB_PDL_PROLOGUE();
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (long long)a.B * a.A) return;
   const int b = (int)(i / a.A);
@@ -203,7 +201,6 @@ __global__ void __launch_bounds__(256) tal_resolve_kernel(const TalArgs a) {
 // ---------------------------------------------------------------------------------------------------------------------
 template <int VEC>
 __global__ void __launch_bounds__(256) tal_scores_kernel(const TalArgs a) {
-  ETB_PDL_PROLOGUE();
   const int per = a.nc / VEC;                                // vectors per anchor
   const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= (long long)a.B * a.A * per) return;
@@ -297,7 +294,6 @@ struct V8Args {
 };
 
 __global__ void __launch_bounds__(256) v8_box_kernel(const V8Args a) {
-  ETB_PDL_PROLOGUE();
   const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;     // grid is padded to a multiple of 4 threads per anchor
   const long long total = (long long)a.B * a.A * 4;
   const bool live = t < total;
@@ -335,7 +331,6 @@ __global__ void __launch_bounds__(256) v8_box_kernel(const V8Args a) {
 }
 
 __global__ void __launch_bounds__(256) v8_cls_kernel(const V8Args a) {
-  ETB_PDL_PROLOGUE();
   const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   const int per = a.nc + 1;
   if (e >= (long long)a.B * a.A * per) return;

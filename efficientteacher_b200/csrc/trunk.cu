@@ -21,7 +21,6 @@ static inline unsigned grid_for(int64_t n, int threads) {
 #define STEM_TP 64
 #define STEM_PITCH 133
 __global__ void __launch_bounds__(256) stem_im2col_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ y, int N, int H, int W, float mul) {
-  ETB_PDL_PROLOGUE();
   __shared__ float sm[18 * STEM_PITCH];
   const int Ho = H / 2, Wo = W / 2;
   const int tiles_w = (Wo + STEM_TP - 1) / STEM_TP;
@@ -74,7 +73,6 @@ extern "C" int etb_stem_im2col(const float* x, void* y_bf16, int32_t N, int32_t 
 // ---- NCHW fp32 <-> NHWC bf16 (simple gather; used at the edges of the trunk and by the tests) ----
 __global__ void __launch_bounds__(256) nchw2nhwc_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ y, int N, int C, int H, int W,
                                                         int cs, int co, float mul) {
-  ETB_PDL_PROLOGUE();
   const int64_t total = (int64_t)N * H * W * C;
   for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (int64_t)gridDim.x * blockDim.x) {
     const int c = (int)(e % C);
@@ -84,7 +82,6 @@ __global__ void __launch_bounds__(256) nchw2nhwc_kernel(const float* __restrict_
   }
 }
 __global__ void __launch_bounds__(256) nhwc2nchw_kernel(const __nv_bfloat16* __restrict__ x, float* __restrict__ y, int N, int C, int H, int W, int cs, int co) {
-  ETB_PDL_PROLOGUE();
   const int64_t total = (int64_t)N * H * W * C;
   for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (int64_t)gridDim.x * blockDim.x) {
     const int w = (int)(e % W), h = (int)((e / W) % H), c = (int)((e / ((int64_t)W * H)) % C), n = (int)(e / ((int64_t)W * H * C));
@@ -114,7 +111,6 @@ __device__ __forceinline__ void bf8_max(uint4& acc, const uint4& v) {
   for (int j = 0; j < 4; ++j) a[j] = __hmax2(a[j], b[j]);
 }
 __global__ void __launch_bounds__(256) sppf_pool_kernel(__nv_bfloat16* __restrict__ buf, int N, int H, int W, int C, int cs) {
-  ETB_PDL_PROLOGUE();
   const int cg = C / 8;
   const int64_t total = (int64_t)N * H * W * cg;
   const uint32_t ninf2 = 0xFF80FF80u;  // bf16 -inf pair (max-pool padding value)
@@ -151,7 +147,6 @@ extern "C" int etb_sppf_pool(void* buf_bf16, int32_t N, int32_t H, int32_t W, in
 // ---- nearest 2x upsample into a channel slice ----
 __global__ void __launch_bounds__(256) upsample2x_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat16* __restrict__ y, int N, int H, int W, int C,
                                                          int xcs, int xco, int ycs, int yco) {
-  ETB_PDL_PROLOGUE();
   const int cg = C / 8;
   const int Ho = 2 * H, Wo = 2 * W;
   const int64_t total = (int64_t)N * Ho * Wo * cg;
@@ -174,7 +169,6 @@ extern "C" int etb_upsample2x_nhwc(const void* x_bf16, void* y_bf16, int32_t N, 
 
 // ---- BN folding + weight packing ----
 __global__ void fold_bn_kernel(const float* g, const float* b, const float* m, const float* v, float eps, float* scale, float* bias, int C) {
-  ETB_PDL_PROLOGUE();
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= C) return;
   const float s = g[c] / sqrtf(v[c] + eps);
@@ -190,7 +184,6 @@ extern "C" int etb_fold_bn(const float* gamma, const float* beta, const float* m
 }
 
 __global__ void __launch_bounds__(256) pack_weight_kernel(const float* __restrict__ w, __nv_bfloat16* __restrict__ o, int Cout, int Cin, int kh, int kw, int Cp) {
-  ETB_PDL_PROLOGUE();
   const int64_t total = (int64_t)Cout * kh * kw * Cp;
   for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (int64_t)gridDim.x * blockDim.x) {
     const int c = (int)(e % Cp);
@@ -207,7 +200,6 @@ extern "C" int etb_pack_weight(const float* w_oihw, void* w_bf16, int32_t Cout, 
 }
 
 __global__ void pack_stem_weight_kernel(const float* __restrict__ w, __nv_bfloat16* __restrict__ o, int Cout) {
-  ETB_PDL_PROLOGUE();
   const int e = blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= Cout * 128) return;
   const int k = e & 127, oc = e >> 7;
@@ -228,7 +220,6 @@ extern "C" int etb_pack_stem_weight(const float* w_oihw, void* w_bf16, int32_t C
 // mode 2: stem [Cout][128] in the etb_stem_im2col K order
 // mode 3: mode 1 negated (dgrad operand of a conv that sits behind a GradReverse)
 __global__ void __launch_bounds__(256) pack_multi_kernel(const EtbPackDesc* __restrict__ descs, const int2* __restrict__ chunks) {
-  ETB_PDL_PROLOGUE();
   const int2 ch = chunks[blockIdx.x];
   const EtbPackDesc d = descs[ch.x];
   const float* __restrict__ w = d.w;
@@ -272,7 +263,6 @@ extern "C" int etb_pack_multi(const EtbPackDesc* descs_dev, const void* chunks_d
 }
 
 __global__ void __launch_bounds__(256) fold_multi_kernel(const EtbFoldDesc* __restrict__ descs) {
-  ETB_PDL_PROLOGUE();
   const EtbFoldDesc d = descs[blockIdx.x];
   for (int c = threadIdx.x; c < d.C; c += 256) {
     const float s = d.gamma[c] / sqrtf(d.var[c] + d.eps);

@@ -19,7 +19,6 @@
 __global__ void __launch_bounds__(VAL_THREADS) val_process_batch_kernel(const float* __restrict__ det, const int* __restrict__ det_cnt, int max_det, int det_ld,
                                                                         const float* __restrict__ labels, int nt, const float* __restrict__ iouv, int T,
                                                                         unsigned char* __restrict__ correct, int* __restrict__ overflow) {
-  ETB_PDL_PROLOGUE();
   __shared__ float lab[VAL_MAX_LABELS][5];     // cls, x1, y1, x2, y2
   __shared__ int nlab;
   __shared__ float biou[VAL_MAX_DET];
@@ -93,7 +92,6 @@ extern "C" int etb_val_process_batch(const float* det, const int32_t* det_cnt, i
 #define MERGE_MAXN 1024
 __global__ void __launch_bounds__(256) nms_boxes_kernel(const float* __restrict__ rows, const int* __restrict__ cnt, int nmax, int ld, float thr,
                                                         float* __restrict__ out, int* __restrict__ out_cnt) {
-  ETB_PDL_PROLOGUE();
   __shared__ int order[MERGE_MAXN];
   __shared__ unsigned char sup[MERGE_MAXN];
   __shared__ int s_keep;

@@ -202,26 +202,15 @@ class YoloV5BackBone(nn.Module):
         self.sppf = SPPF(c5, c5, 5, act)
         self.out_shape = {'C3_size': c3, 'C4_size': c4, 'C5_size': c5}
 
-    grad_marks = None     # (fn_after_stage5_2, fn_after_stage4_2): parallel.GradMarkFn callbacks set by the trainer (WORLD_SIZE > 1)
-
-    def _mark(self, x, k):
-        """autograd mark on the activation that separates two chunks of the gradient arena: when its backward runs, the
-        gradients of every layer after it are complete and their all-reduce can start (parallel.GradArena.chunk_ready)"""
-        fn = self.grad_marks[k] if (self.grad_marks and x.requires_grad) else None
-        if fn is None:
-            return x
-        from .parallel import GradMarkFn
-        return GradMarkFn.apply(x, fn)
-
     def forward(self, x):
         x = self.stage2_2(self.stage2_1(self.stage1(x)))
         c3 = self.stage3_2(self.stage3_1(x))
         if self.stage4_1.glue(c3):
             _fan_out(c3)          # consumed by stage4_1 and by the neck's concat (JoinFn lateral)
-        c4 = self.stage4_2(self._mark(self.stage4_1(c3), 1))
+        c4 = self.stage4_2(self.stage4_1(c3))
         if self.stage5_1.glue(c4):
             _fan_out(c4)
-        return c3, c4, self.sppf(self.stage5_2(self._mark(self.stage5_1(c4), 0)))
+        return c3, c4, self.sppf(self.stage5_2(self.stage5_1(c4)))
 
 
 class YoloV5Neck(nn.Module):

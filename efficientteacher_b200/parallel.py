@@ -1,23 +1,17 @@
-"""Data parallelism of the SSOD step (SURVEY.md 8e): one process per GPU, NCCL over NVLink, and exactly ONE collective per
-step -- a SUM all-reduce of the flat fp32 gradient arena (191.8 MB for YOLOv5l-SSOD).
+"""Data parallelism of the SSOD step (SURVEY.md 8e): one process per GPU, NCCL over NVLink, and two collectives per step --
+a SUM all-reduce of the flat fp32 gradient arena (191.8 MB for YOLOv5l-SSOD) after backward, and a broadcast of the
+student's BatchNorm running statistics before its forward.
 
 The reference wraps the student in DDP (trainer/trainer.py:313), multiplies both losses by WORLD_SIZE
 (trainer/ssod_trainer.py:638-639,647-648) and lets DDP average the bucketed gradients: mean(W*g_r) == sum(g_r).  Here the
-losses are left unscaled and the arena is summed once, after backward.  BatchNorm statistics stay per rank (SyncBN is off
-in every shipped config) and the teacher EMA is updated locally from the identical post-all-reduce weights, so no other
-communication exists.
+losses are left unscaled and the arena (GradArena) is summed once, after backward.  BatchNorm statistics stay per rank
+(SyncBN is off in every shipped config) and the teacher EMA is updated locally from the identical post-all-reduce weights.
 
-Two refinements on top of the single all-reduce:
-  * overlap (SURVEY.md 5b): the arena is laid out in BACKWARD-COMPLETION order (reverse registration order: netD, head,
-    neck ... stem) and cut into a few chunks at module boundaries; autograd marks placed at those boundaries (GradMarkFn)
-    fire when every gradient of a chunk has been enqueued, and the chunk's ncclAllReduce is issued on a communication stream
-    behind an event -- the collective overlaps the rest of the backward pass.  All of it is captured into the step's CUDA
-    graph (cross-stream dependencies), so no host round-trip sits between backward and the optimizer.
-  * BatchNorm buffers (SURVEY.md 8e caveat 2): the reference's DDP runs with broadcast_buffers=True, i.e. at the start of
-    every forward rank 0's running_mean / running_var overwrite every rank's.  BnBufferSync keeps all running statistics of
-    the student in ONE flat buffer and broadcasts it from rank 0 before the student forward (60,151 floats: one small NCCL
-    broadcast), reproducing that.  (The reference's per-rank teachers are therefore NOT identical across ranks either: each
-    rank's EMA sees 0.97 * rank0's statistics + 0.03 * its own batch's; only rank 0's teacher is validated / saved.)"""
+BatchNorm buffers (SURVEY.md 8e caveat 2): the reference's DDP runs with broadcast_buffers=True, i.e. at the start of every
+forward rank 0's running_mean / running_var overwrite every rank's.  BnBufferSync keeps all running statistics of the
+student in ONE flat buffer and broadcasts it from rank 0 before the student forward (60,151 floats: one small NCCL
+broadcast), reproducing that.  (The reference's per-rank teachers are therefore NOT identical across ranks either: each
+rank's EMA sees 0.97 * rank0's statistics + 0.03 * its own batch's; only rank 0's teacher is validated / saved.)"""
 import torch
 
 
@@ -35,10 +29,8 @@ class GradArena:
             o += (p.numel() + cls.ALIGN - 1) // cls.ALIGN * cls.ALIGN
         return offs, o
 
-    def __init__(self, params, device=None, reverse=False, chunk_ends=None):
-        """reverse: lay the arena out in reverse parameter order (= the order in which backward completes the gradients).
-        chunk_ends: optional list of parameter tensors; a chunk boundary is placed right AFTER each of them (in arena
-        order), giving len(chunk_ends)+1 contiguous chunks for the overlapped all-reduce."""
+    def __init__(self, params, device=None, reverse=False):
+        """reverse: lay the arena out in reverse parameter order (= the order in which backward completes the gradients)."""
         self.params = [p for p in params if p.requires_grad]
         if reverse:
             self.params = self.params[::-1]
@@ -47,62 +39,11 @@ class GradArena:
         self.flat = torch.zeros(n, dtype=torch.float32, device=dev)
         for p, o in zip(self.params, self.offsets):
             p.grad = self.flat[o:o + p.numel()].view_as(p)
-        # chunk k = flat[bounds[k]:bounds[k+1]]
-        self.bounds = [0]
-        if chunk_ends:
-            ends = {id(t) for t in chunk_ends}
-            for p, o in zip(self.params, self.offsets):
-                if id(p) in ends:
-                    self.bounds.append(o + (p.numel() + self.ALIGN - 1) // self.ALIGN * self.ALIGN)
-        self.bounds.append(n)
-        self.bounds = sorted(set(self.bounds))
-        self._works, self._comm, self._next = [], None, 0
         self.average = False    # True: ncclAvg instead of ncclSum (same collective, same cost); see SSODTrainerStep.GRAD_REDUCE
 
     def _op(self):
         import torch.distributed as dist
         return dist.ReduceOp.AVG if self.average else dist.ReduceOp.SUM
-
-    def n_chunks(self):
-        return len(self.bounds) - 1
-
-    # ---- overlapped, chunked all-reduce (see the module docstring) ----
-    def begin_step(self):
-        self._works, self._next = [], 0
-
-    def chunk_ready(self, k, world_size, extra_stream=None, group=None):
-        """every gradient of chunks <= k has been enqueued (on the current stream and, for the weight gradients, on
-        `extra_stream`): issue their all-reduce on the communication stream, behind events on both."""
-        if world_size <= 1:
-            return
-        import torch.distributed as dist
-        cur = torch.cuda.current_stream(self.flat.device)
-        if self._comm is None:
-            self._comm = torch.cuda.Stream(self.flat.device)
-        for st in (cur, extra_stream):
-            if st is not None:
-                ev = torch.cuda.Event()
-                ev.record(st)
-                self._comm.wait_event(ev)
-        with torch.cuda.stream(self._comm):
-            while self._next <= k and self._next < self.n_chunks():
-                a, b = self.bounds[self._next], self.bounds[self._next + 1]
-                self._works.append(dist.all_reduce(self.flat[a:b], op=self._op(), group=group, async_op=True))
-                self._next += 1
-
-    def finish(self, world_size, extra_stream=None, group=None):
-        """all-reduce whatever chunks are still outstanding and make the current stream wait for all of them"""
-        if world_size <= 1:
-            return self.flat
-        self.chunk_ready(self.n_chunks() - 1, world_size, extra_stream, group)
-        for w in self._works:
-            w.wait()
-        cur = torch.cuda.current_stream(self.flat.device)
-        ev = torch.cuda.Event()
-        ev.record(self._comm)
-        cur.wait_event(ev)
-        self._works = []
-        return self.flat
 
     def zero(self):
         self.flat.zero_()
@@ -119,22 +60,6 @@ class GradArena:
             import torch.distributed as dist
             dist.all_reduce(self.flat, op=self._op(), group=group)
         return self.flat
-
-
-class GradMarkFn(torch.autograd.Function):
-    """identity in forward; in backward calls `fn()` -- placed on an activation that separates two groups of layers, it fires
-    exactly when autograd has finished (enqueued) every node created after it, i.e. when the gradients of all later layers
-    are complete (the engine runs ready nodes in reverse creation order)."""
-
-    @staticmethod
-    def forward(ctx, x, fn):
-        ctx.fn = fn
-        return x.view_as(x)
-
-    @staticmethod
-    def backward(ctx, g):
-        ctx.fn()
-        return g, None
 
 
 class BnBufferSync:

@@ -114,33 +114,8 @@ class SSODTrainerStep:
     # ---- gradient arena: all student gradients live in one flat fp32 buffer -> ONE all-reduce per step ----
     def _ensure_arena(self):
         if self._arena is None:
-            bb = self.model.backbone
-            # backward-completion order + chunk boundaries at the two autograd marks of YoloV5BackBone.forward:
-            # [netD, head, neck, sppf, stage5_2] | [stage5_1, stage4_2] | [stage4_1 ... stem]
-            self._arena = GradArena(self.model.parameters(), self.device, reverse=True,
-                                    chunk_ends=[bb.stage5_2.cv1.conv.weight, bb.stage4_2.cv1.conv.weight])
-            if self.WORLD_SIZE > 1:
-                from . import autograd_conv as ac
-                side = lambda: ac.WGRAD_SIDE["stream"] if ac.WGRAD_SIDE["dirty"] else None  # noqa: E731
-                bb.grad_marks = tuple((lambda k=k: self._arena.chunk_ready(k, self.WORLD_SIZE, side()) if self._overlap_comm() else None)
-                                      for k in (0, 1))
+            self._arena = GradArena(self.model.parameters(), self.device, reverse=True)   # backward-completion order
         return self._arena
-
-    # Communication modes (WORLD_SIZE > 1).  Default = the round-1 scheme that the 1->8 GPU scaling runs were measured with: ONE
-    # eager all-reduce of the arena between graph A and graph B, plus one eager broadcast of rank 0's BN statistics before the
-    # step.  ETB_COMM_OVERLAP=1: the all-reduce is issued in 3 chunks from autograd marks during backward on a communication
-    # stream (eager steps); ETB_COMM_IN_GRAPH=1 additionally captures the NCCL calls inside graph A (no host round-trip).
-    COMM_OVERLAP = os.environ.get("ETB_COMM_OVERLAP", "0") == "1"
-    COMM_IN_GRAPH = os.environ.get("ETB_COMM_IN_GRAPH", "0") == "1"
-
-    def _overlap_comm(self):
-        """the chunked all-reduce may run INSIDE backward only when every backward is followed by an optimizer step
-        (accumulate == 1): gradients accumulate in the arena across iterations, so they must be reduced once per step"""
-        if self.WORLD_SIZE <= 1 or not (self.fixed_accumulate or max(round(64 / self.batch_size), 1) == 1):
-            return False
-        if torch.cuda.is_current_stream_capturing():
-            return self.COMM_IN_GRAPH
-        return self.COMM_OVERLAP or self.COMM_IN_GRAPH
 
     # "sum" = the reference (loss * WORLD_SIZE, then DDP's mean: trainer/ssod_trainer.py:638-648).  "avg" (ncclAvg: the same
     # collective at the same cost) is for synthetic benchmarks only: with SUM the effective learning rate grows with the world
@@ -149,14 +124,11 @@ class SSODTrainerStep:
     GRAD_REDUCE = os.environ.get("ETB_GRAD_REDUCE", "sum")
 
     def _allreduce_grads(self):
-        """WORLD_SIZE > 1: all-reduce of the gradient arena (the chunks that were not already issued during backward)"""
+        """WORLD_SIZE > 1: one all-reduce of the whole gradient arena"""
         if self.WORLD_SIZE <= 1:
             return
         self._arena.average = (self.GRAD_REDUCE == "avg")
-        if self._arena._next == 0 and not (self.COMM_OVERLAP or self.COMM_IN_GRAPH):
-            self._arena.all_reduce_sum(self.WORLD_SIZE)          # one collective over the whole arena
-        else:
-            self._arena.finish(self.WORLD_SIZE)
+        self._arena.all_reduce_sum(self.WORLD_SIZE)
 
     def _bn_broadcast(self):
         """DDP broadcast_buffers=True: rank 0's BN running statistics overwrite every rank's before each forward"""
@@ -173,7 +145,6 @@ class SSODTrainerStep:
 
     def _backward(self, loss):
         self._ensure_arena()
-        self._arena.begin_step()
         from . import autograd_conv as ac
         ac.backward(loss, side=self.WGRAD_SIDE_STREAM)   # weight-gradient branch on a side stream, joined before returning
         self._mark("backward")
@@ -238,7 +209,7 @@ class SSODTrainerStep:
                        host_pseudo_labels=False, _stop_after_backward=False):
         n_img = imgs.shape[0]
         self._mark("start")
-        if self.WORLD_SIZE > 1 and (self.COMM_IN_GRAPH or not torch.cuda.is_current_stream_capturing()):
+        if self.WORLD_SIZE > 1 and not torch.cuda.is_current_stream_capturing():
             self._bn_broadcast()         # (captured steps: train_instance_graphed issues it before the replay)
         # The teacher forward + NMS + pseudo-label transform feed nothing but the unsupervised loss, and the student forward
         # does not depend on them: with the device-resident pseudo labels they run on a side stream, concurrently with the
@@ -299,10 +270,8 @@ class SSODTrainerStep:
         # DDP: loss*WORLD_SIZE then gradient mean == plain SUM all-reduce of per-rank gradients (no scaling here)
         loss = sup_loss + un_sup_loss * self.cfg.SSOD.teacher_loss_weight
         self._mark("losses")
-        if _stop_after_backward:         # captured graph A ends here; with accumulate == 1 it also contains the (overlapped) all-reduce
+        if _stop_after_backward:         # captured graph A ends here
             self._backward(loss)
-            if self._overlap_comm():
-                self._allreduce_grads()
             return loss.detach()
         self.update_optimizer(loss, ni)
         self._mark("optimizer_ema")
@@ -335,7 +304,6 @@ class SSODTrainerStep:
         g["us"].copy_(unlabeled_imgs, non_blocking=True)
         g["uw"].copy_(unlabeled_imgs_ori, non_blocking=True)
         g["Ms"].copy_(unlabeled_M, non_blocking=True)
-        comm_in_a = self.WORLD_SIZE > 1 and self.COMM_IN_GRAPH and (self.fixed_accumulate or max(round(64 / self.batch_size), 1) == 1)
         # everything the host contributes to this iteration is enqueued BEFORE graph A, so that A, the all-reduce and B follow
         # each other on the stream without a host gap: accumulate / lr / momentum of iteration ni (host scalars), and -- when
         # the optimizer is due -- the EMA decays and the SGD hyper-parameters (stream-ordered copies: the previous replay of B
@@ -346,13 +314,10 @@ class SSODTrainerStep:
             # pageable source: the runtime stages the 16 bytes before returning, so the next step cannot overwrite them early
             self._ema_scalars_dev.copy_(torch.tensor(ema_scalars(d1, d2), dtype=torch.float32))
             self.optimizer.refresh_hyper()   # lr / momentum of this step -> device memory read by the captured SGD kernel
-        if self.WORLD_SIZE > 1 and not self.COMM_IN_GRAPH:
-            self._bn_broadcast()
+        self._bn_broadcast()
         g["graph"].replay()
         if due:
-            if self.WORLD_SIZE > 1 and not comm_in_a:
-                self._arena.begin_step()
-                self._allreduce_grads()      # one SUM all-reduce per optimizer step, between the two graphs (enqueued, no host sync)
+            self._allreduce_grads()          # one SUM all-reduce per optimizer step, between the two graphs (enqueued, no host sync)
             g["graph_b"].replay()
             self.last_opt_step = ni
         if hasattr(self.pseudo_label_creator, "stage_detections"):   # LabelMatch: the captured step cannot stage its detections itself
@@ -400,8 +365,7 @@ class SSODTrainerStep:
         with torch.cuda.stream(side):
             for _ in range(2):
                 self.train_instance(st["imgs"], st["targets"], st["us"], st["uw"], None, st["Ms"], ni, _stop_after_backward=True)
-                if self._arena._next == 0:      # not already reduced inside train_instance (overlapped mode)
-                    self._allreduce_grads()
+                self._allreduce_grads()
                 self._warmup(ni)
                 self._step_and_ema()          # the optimizer + EMA branch is exercised (and later captured) unconditionally
         torch.cuda.current_stream(dev).wait_stream(side)
@@ -469,9 +433,6 @@ class SupTrainerStep:
     _ensure_arena = SSODTrainerStep._ensure_arena
     _bn_broadcast = SSODTrainerStep._bn_broadcast
     _bn_sync = None
-
-    def _overlap_comm(self):          # the supervised step keeps the single all-reduce after backward
-        return False
 
     def _forward_backward(self, imgs, targets):
         if self.WORLD_SIZE > 1 and not torch.cuda.is_current_stream_capturing():

@@ -387,21 +387,6 @@ int etb_val_process_batch(const float* det, const int32_t* det_cnt, int32_t B, i
 int etb_nms_boxes(const float* rows, const int32_t* cnt, int32_t B, int32_t nmax, int32_t ld, float iou_thres, float* out,
                   int32_t* out_cnt, void* stream);
 
-/* fused (cooperative, one launch) training BatchNorm + activation, forward and backward: statistics -> finalize -> apply with
- * two grid barriers inside ONE co-resident grid (csrc/bn.cu).  Same arithmetic as the three-kernel sequences above.
- *   rows = etb_bn_fused_rows(M, C, which) is the grid size AND the row count of `partials` ([rows][2][C] floats);
- *   barrier: 2 x uint32 zero-initialised once by the caller and reused (self-resetting); one per stream.
- *   forward : stats [4][C] = scale, shift, mean, invstd (kept for the backward); running statistics updated in place.
- *   backward: sums [2][C] scratch; dgamma / dbeta written, or added in place when accumulate != 0. */
-int32_t etb_bn_fused_rows(int64_t M, int32_t C, int32_t which);
-int etb_bn_fwd_fused(const void* y_bf16, int64_t M, int32_t C, int32_t y_cstride, const float* gamma, const float* beta,
-                     float eps, float momentum, float* running_mean, float* running_var, float* stats,
-                     const void* res_bf16, int32_t res_cstride, void* out_bf16, int32_t out_cstride, int32_t act,
-                     float* partials, int32_t rows, uint32_t* barrier, void* stream);
-int etb_bn_bwd_fused(const void* da_bf16, const void* y_bf16, const float* stats, int64_t M, int32_t C, int32_t da_cstride,
-                     int32_t y_cstride, int32_t dy_cstride, int32_t act, void* dy_bf16, float* sums, float* dgamma,
-                     float* dbeta, int32_t accumulate, float* partials, int32_t rows, uint32_t* barrier, void* stream);
-
 /* ---------------------------------------------------------------------------------------------
  * Anchor-free (YOLOv8) pieces -- SURVEY.md section 8f row 5.  The reference defines no end-to-end step for this head
  * (models/loss/tal_loss.py cannot be imported, trainer/ssod_trainer.py:598-606 rejects it): these are the importable

@@ -27,9 +27,8 @@ def _worker(rank, world, port, out):
     dist.init_process_group("gloo", rank=rank, world_size=world)
     from efficientteacher_b200.parallel import BnBufferSync, GradArena
     net = _net()
-    # backward-completion order + one chunk boundary, like the trainer builds it
-    arena = GradArena(net.parameters(), reverse=True, chunk_ends=[net[3].weight])
-    assert arena.n_chunks() == 2 and arena.bounds[0] == 0 and arena.bounds[-1] == arena.flat.numel()
+    # backward-completion order, like the trainer builds it
+    arena = GradArena(net.parameters(), reverse=True)
     assert arena.params[0] is net[3].bias and arena.params[-1] is net[0].weight
     sync = BnBufferSync(net)
     assert net[1].running_mean.data_ptr() == sync.flat.data_ptr() and "running_var" in dict(net[1].named_buffers())

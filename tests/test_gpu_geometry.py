@@ -335,13 +335,11 @@ def test_wgrad_nan_poisoned_slices(Cin, Cout, k, s):
     _check_per_channel(dw, _ref_wgrad(x, dy, Cout, k, s, p), 5e-4, "wgrad")
 
 
-@pytest.mark.parametrize("one_launch", [True, False])
 @pytest.mark.parametrize("C_", [32, 64])
-def test_bn_nan_poisoned_slices(C_, one_launch, monkeypatch):
+def test_bn_nan_poisoned_slices(C_):
     """training BatchNorm + SiLU forward (y / out / residual slices) and backward (da / y slices, dy into a wider buffer,
     dgamma / dbeta added into existing gradients) against float64 autograd of F.batch_norm"""
     from efficientteacher_b200 import convops as co
-    monkeypatch.setattr(co, "BN_FUSED", one_launch)
     N, H, W, eps, mom = 2, 11, 20, 1e-3, 0.03
     y = _bf((N, C_, H, W), 81, 2.0) + 0.25
     y = y.to(torch.bfloat16).float()
