@@ -8,11 +8,8 @@ convs (models/head/yolov5_head.py:55) and netD.conv1 (models/detector/yolo_ssod.
 """
 import torch
 
-from . import _lib
 from . import convops as co
 
-
-ACCUMULATE_INTO_GRAD = True
 
 # Optional side stream for the weight-gradient branch.  In backward, wgrad (+ its split-K reduce) of a layer depends only on
 # that layer's dy and feeds nothing but the gradient arena, while the critical path continues dgrad -> previous layer's BN
@@ -57,23 +54,31 @@ def wgrad_side_join():
         S["dirty"] = False
 
 
+def _inplace_nhwc(t, C_):
+    """(NHWC view, pixel stride) of a bf16 NCHW-shaped tensor that is physically NHWC (possibly a channel slice), else None"""
+    N, C2, H, W = t.shape
+    if t.dtype != torch.bfloat16 or C2 != C_:
+        return None
+    sN, sC, sH, sW = t.stride()
+    if sC == 1 and sW >= C_ and sW % 8 == 0 and sH == W * sW and sN == H * W * sW and t.data_ptr() % 16 == 0:
+        return t.permute(0, 2, 3, 1), sW
+    return None
+
+
 def _as_nhwc(t, C_):
     """(view [N,H,W,C] bf16 whose channel stride may exceed C, channel_stride) for an NCHW-shaped tensor; copies only if
     the layout is not NHWC.  A channel-slice of a channels_last tensor (what torch.cat's backward hands out) is used in
     place: the kernels take the pixel stride separately and never touch channels outside the slice."""
     N, C2, H, W = t.shape
     assert C2 == C_
-    if t.dtype != torch.bfloat16:
-        t = t.to(torch.bfloat16)
-    sN, sC, sH, sW = t.stride()
-    cs = sW
-    ok = sC == 1 and cs >= C_ and cs % 8 == 0 and sH == W * cs and sN == H * W * cs and t.data_ptr() % 16 == 0
-    if not ok:
+    t = t.to(torch.bfloat16)
+    v = _inplace_nhwc(t, C_)
+    if v is None:
         t = t.contiguous(memory_format=torch.channels_last)
-        cs = C_
         if t.stride() != (H * W * C_, 1, W * C_, C_):     # degenerate shapes (H=W=1 ...): force the NHWC strides
             t = t.permute(0, 2, 3, 1).contiguous().permute(0, 3, 1, 2)
-    return t.permute(0, 2, 3, 1), cs
+        v = t.permute(0, 2, 3, 1), C_
+    return v
 
 
 def _empty_cl(N, C_, H, W, device):
@@ -83,17 +88,17 @@ def _empty_cl(N, C_, H, W, device):
 
 
 def _nhwc_of(t):
-    N, C_, H, W = t.shape
-    v = t.permute(0, 2, 3, 1)
-    if v.stride() != (H * W * C_, W * C_, C_, 1):       # degenerate sizes: channels_last strides are ambiguous
+    """dense NHWC view of a tensor from _empty_cl"""
+    v = _inplace_nhwc(t, t.shape[1])
+    if v is None or v[1] != t.shape[1]:
         raise RuntimeError("unexpected channels_last strides %s for %s" % (t.stride(), tuple(t.shape)))
-    return v
+    return v[0]
 
 
 class StemInput:
     """The student's input batch as the stem sees it: one or several [n_i,3,H,W] tensors (uint8 straight from the loaders,
     or fp32 already scaled) that are logically concatenated along the batch (trainer/ssod_trainer.py:620 torch.cat) and
-    divided by `div` (:694-696 `.float() / 255`).  Deliberately NOT a tensor: ConvBnActFn receives it as an opaque argument
+    divided by `div` (:694-696 `.float() / 255`).  Deliberately NOT a tensor: the stem's Function receives it as an opaque argument
     and the im2col kernel reads every part in place -- neither the cat nor the fp32 image is ever materialised."""
 
     def __init__(self, parts, div=None):
@@ -202,6 +207,14 @@ class FanIn:
         """the FanIn attached to tensor x by its producer module (None if x has a single consumer)"""
         return getattr(x, "_etb_fan", None) if x.requires_grad else None
 
+    @staticmethod
+    def join(x):
+        """register a native consumer of x in forward; returns x's FanIn (None if x has a single consumer)"""
+        f = FanIn.of(x)
+        if f is not None:
+            f.n += 1
+        return f
+
     def done(self):
         self.k += 1
         if self.k < self.n:
@@ -217,27 +230,44 @@ class FanIn:
     def add_dgrad(self, run, N, C_, H, W, device):
         """convolution contribution: run(out_nhwc, out_cstride, accumulate) launches the dgrad"""
         if self.buf is None:
-            self.buf = _empty_cl(N, C_, H, W, device)
-            run(_nhwc_of(self.buf), C_, False)
+            self.buf = input_grad(None, run, N, C_, H, W, device)
         else:
             v = _inplace_nhwc(self.buf, C_)
             if v is None:                      # layout the kernel cannot address in place: out-of-place fallback
-                dx = _empty_cl(N, C_, H, W, device)
-                run(_nhwc_of(dx), C_, False)
-                self.buf = self.buf + dx
+                self.buf = self.buf + input_grad(None, run, N, C_, H, W, device)
             else:
                 run(v[0], v[1], True)
         return self.done()
 
 
-def _inplace_nhwc(t, C_):
-    """(NHWC view, pixel stride) of a bf16 NCHW-shaped tensor that is physically NHWC (possibly a channel slice), else None"""
-    N, C2, H, W = t.shape
-    if t.dtype != torch.bfloat16 or C2 != C_:
-        return None
-    sN, sC, sH, sW = t.stride()
-    if sC == 1 and sW >= C_ and sW % 8 == 0 and sH == W * sW and sN == H * W * sW and t.data_ptr() % 16 == 0:
-        return t.permute(0, 2, 3, 1), sW
+def input_grad(fan, run, N, C_, H, W, device):
+    """the input gradient a native backward hands to autograd, from the dgrad launcher run(out_nhwc, out_cstride,
+    accumulate): a fresh tensor, or -- when the input's gradient fans in -- this contribution to the FanIn buffer"""
+    if fan is not None:
+        return fan.add_dgrad(run, N, C_, H, W, device)
+    dx = _empty_cl(N, C_, H, W, device)
+    run(_nhwc_of(dx), C_, False)
+    return dx
+
+
+def _arena_grad(p):
+    """p.grad when it is the contiguous fp32 gradient-arena view the kernels may accumulate into, else None"""
+    g = p.grad
+    return g if (g is not None and g.dtype == torch.float32 and g.is_contiguous()) else None
+
+
+def weight_grad(p, fn, keep=None):
+    """the gradient of parameter p a native backward hands to autograd, from the launcher fn(accumulate_into).  When p.grad
+    is a gradient-arena view (trainer.GradArena) the result is added into it in place and autograd gets None (no separate
+    AccumulateGrad pass, no temporary).  keep: the operands of a weight-gradient conv; with the side stream on, an
+    in-place launch goes there and they stay alive until the join.  Launchers without `keep` stay on the current stream."""
+    tgt = _arena_grad(p)
+    if tgt is None:
+        return fn(None)
+    if keep is not None and WGRAD_SIDE["on"]:
+        wgrad_side_run(lambda: fn(tgt), keep)
+    else:
+        fn(tgt)
     return None
 
 
@@ -256,10 +286,7 @@ class JoinFn(torch.autograd.Function):
         off, splits = 0, []
         ctx.fans = []
         for p, cp in zip(parts, copy_flags):
-            fan = FanIn.of(p) if cp else None      # a copied-in part (backbone feature, lateral) may have other consumers
-            if fan is not None:
-                fan.n += 1
-            ctx.fans.append(fan)
+            ctx.fans.append(FanIn.join(p) if cp else None)      # a copied-in part (backbone feature, lateral) may have other consumers
             C_ = p.shape[1]
             if cp:
                 pb, pcs = _as_nhwc(p, C_)
@@ -289,9 +316,7 @@ class UpsampleIntoFn(torch.autograd.Function):
     def forward(ctx, x, dest, coff):
         N, C_, H, W = x.shape
         xb, xcs = _as_nhwc(x, C_)
-        out, _ = _slice_nhwc(dest, coff, C_)
-        _lib.check(_lib.lib().etb_upsample2x_nhwc(_lib.ptr(xb), _lib.ptr(out), N, H, W, C_, xcs, 0, dest.Ct, 0, _lib.stream_ptr()),
-                   "etb_upsample2x_nhwc")
+        co.upsample2x(xb, C_, dest.buf.permute(0, 2, 3, 1), coff, x_cstride=xcs)
         ctx.geom = (N, C_, H, W)
         return dest.slice(coff, C_)
 
@@ -335,38 +360,65 @@ class SppfPoolFn(torch.autograd.Function):
         return dx, None
 
 
+def _conv_forward(ctx, x, weight, stride, pad, is_stem, wp, wd):
+    """The convolution shared by ConvFn and ConvBnActFn: (operand saved for backward, raw output y as a channels_last
+    [N,Cout,Ho,Wo] bf16 tensor).  The stem (6x6 s2 p2 on the image, a StemInput or an fp32 tensor) runs as im2col (K=108
+    padded to 128) + pointwise GEMM and saves the im2col instead of the image.  wp / wd: operands from
+    Model.pack_weights(), else packed here."""
+    Cout = weight.shape[0]
+    if is_stem:
+        xs = x.im2col() if isinstance(x, StemInput) else co.stem_im2col(x.float(), 1.0)
+        xb, xcs, Cin, k, st, pd = xs, 128, 128, 1, 1, 0
+        wp = co.pack_stem_weight(weight) if wp is None else wp
+    else:
+        xs, Cin, k, st, pd = x, weight.shape[1], weight.shape[2], stride, pad
+        xb, xcs = _as_nhwc(x, Cin)
+        wp = co.pack_weight(weight) if wp is None else wp
+    N, H, W = xb.shape[:3]
+    y = _empty_cl(N, Cout, (H + 2 * pd - k) // st + 1, (W + 2 * pd - k) // st + 1, xb.device)
+    co.conv_fwd(xb, wp, Cin, Cout, k, st, pd, None, None, None, x_cstride=xcs, out=_nhwc_of(y))
+    ctx.conv = (stride, pad, is_stem, wd)
+    return xs, y
+
+
+def _conv_backward(ctx, xs, weight, dy, dycs, fan):
+    """(dx, dW) of the convolution from dy [N,Ho,Wo,*] bf16 NHWC (pixel stride dycs): dgrad, then wgrad.  The image
+    needs no gradient: the stem runs only the wgrad, on the saved im2col."""
+    stride, pad, is_stem, wd = ctx.conv
+    Cout = weight.shape[0]
+    dx = dw = None
+    if is_stem:
+        xb, xcs, Cin, k, stride, pad = xs, 128, 128, 1, 1, 0
+    else:
+        Cin, k = weight.shape[1], weight.shape[2]
+        if ctx.needs_input_grad[0]:
+            N, _, H, W = xs.shape
+            wd = co.pack_weight_dgrad(weight, stride, pad) if wd is None else wd
+            dx = input_grad(fan, lambda o, ocs, acc: co.conv_dgrad(dy, wd, N, H, W, Cin, Cout, k, stride, pad, out=o, out_cstride=ocs,
+                                                                   accumulate=acc, dy_cstride=dycs), N, Cin, H, W, dy.device)
+        xb, xcs = _as_nhwc(xs, Cin)
+    if ctx.needs_input_grad[1]:
+        dw = weight_grad(weight, lambda into: co.conv_wgrad(xb, dy, Cin, Cout, k, stride, pad, stem=is_stem, x_cstride=xcs,
+                                                            dy_cstride=dycs, accumulate_into=into), (xs, xb, dy))
+    return dx, dw
+
+
 class ConvFn(torch.autograd.Function):
-    """y = conv2d(x, w) (no bias, no activation), bf16 channels_last in / out."""
+    """y = conv2d(x, w) (no bias, no activation), bf16 channels_last out: the Conv modules whose BatchNorm width the fused
+    kernels do not cover run it under torch BatchNorm + activation."""
 
     @staticmethod
-    def forward(ctx, x, weight, stride, pad):
-        Cout, Cin, k, _ = weight.shape
-        xb, xcs = _as_nhwc(x, Cin)
-        wp = co.pack_weight(weight)
-        N, _, H, W = x.shape
-        Ho, Wo = (H + 2 * pad - k) // stride + 1, (W + 2 * pad - k) // stride + 1
-        y = _empty_cl(N, Cout, Ho, Wo, x.device)
-        co.conv_fwd(xb, wp, Cin, Cout, k, stride, pad, None, None, None, x_cstride=xcs, out=_nhwc_of(y))
-        ctx.save_for_backward(x, weight)
-        ctx.geom = (stride, pad)
+    def forward(ctx, x, weight, stride, pad, is_stem, wp=None, wd=None):
+        xs, y = _conv_forward(ctx, x, weight, stride, pad, is_stem, wp, wd)
+        ctx.save_for_backward(xs, weight)
         return y
 
     @staticmethod
     def backward(ctx, dy):
-        x, weight = ctx.saved_tensors
-        stride, pad = ctx.geom
-        Cout, Cin, k, _ = weight.shape
-        N, _, H, W = x.shape
-        dyb, dycs = _as_nhwc(dy, Cout)
-        dx = dw = None
-        if ctx.needs_input_grad[0]:
-            wd = co.pack_weight_dgrad(weight, stride, pad)
-            dx = _empty_cl(N, Cin, H, W, dy.device)
-            co.conv_dgrad(dyb, wd, N, H, W, Cin, Cout, k, stride, pad, dy_cstride=dycs, out=_nhwc_of(dx))
-        if ctx.needs_input_grad[1]:
-            xb, xcs = _as_nhwc(x, Cin)
-            dw = co.conv_wgrad(xb, dyb, Cin, Cout, k, stride, pad, x_cstride=xcs, dy_cstride=dycs)
-        return dx, dw, None, None
+        xs, weight = ctx.saved_tensors
+        dyb, dycs = _as_nhwc(dy, weight.shape[0])
+        dx, dw = _conv_backward(ctx, xs, weight, dyb, dycs, None)
+        return dx, dw, None, None, None, None, None
 
 
 class ConvBnActFn(torch.autograd.Function):
@@ -379,32 +431,14 @@ class ConvBnActFn(torch.autograd.Function):
                 wp=None, wd=None, res=None, dest=None, coff=0):
         """res: optional shortcut tensor added after the activation (Bottleneck, common.py:499); dest/coff: optional
         CatBuf slice the activation is written into (the returned tensor is then that slice)."""
-        Cout = weight.shape[0]
-        ctx.wd = wd
+        ctx.fan = FanIn.join(x)
+        ctx.res_fan = FanIn.join(res) if res is not None else None
         ctx.has_res = res is not None
-        ctx.fan = None if is_stem else FanIn.of(x)
-        ctx.res_fan = FanIn.of(res) if res is not None else None
-        for f in (ctx.fan, ctx.res_fan):
-            if f is not None:
-                f.n += 1
-        if is_stem:
-            xb = x.im2col() if isinstance(x, StemInput) else co.stem_im2col(x.float(), 1.0)   # [N,H/2,W/2,128]; saved instead of the image
-            xcs, Cin, k, st, pd = 128, 128, 1, 1, 0
-            if wp is None:
-                wp = co.pack_stem_weight(weight)
-            N, Ho, Wo = xb.shape[0], xb.shape[1], xb.shape[2]
-        else:
-            Cin, k = weight.shape[1], weight.shape[2]
-            xb, xcs = _as_nhwc(x, Cin)
-            st, pd = stride, pad
-            if wp is None:
-                wp = co.pack_weight(weight)
-            N, _, H, W = x.shape
-            Ho, Wo = (H + 2 * pd - k) // st + 1, (W + 2 * pd - k) // st + 1
-        y = torch.empty((N, Ho, Wo, Cout), dtype=torch.bfloat16, device=x.device)
-        co.conv_fwd(xb, wp, Cin, Cout, k, st, pd, None, None, None, x_cstride=xcs, out=y)
+        xs, y = _conv_forward(ctx, x, weight, stride, pad, is_stem, wp, wd)
+        y = _nhwc_of(y)
+        N, Ho, Wo, Cout = y.shape
         if dest is None:
-            a = _empty_cl(N, Cout, Ho, Wo, x.device)
+            a = _empty_cl(N, Cout, Ho, Wo, y.device)
             ab, acs = _nhwc_of(a), Cout
         else:
             a = dest.slice(coff, Cout)
@@ -412,82 +446,24 @@ class ConvBnActFn(torch.autograd.Function):
         rb, rcs = _as_nhwc(res, Cout) if res is not None else (None, None)
         _, stats = co.bn_forward(y, Cout, gamma.detach(), beta.detach(), running_mean, running_var, eps, momentum, act, out=ab,
                                  out_cstride=acs, res=rb, res_cstride=rcs)
-        ctx.save_for_backward(xb if is_stem else x, weight, y, stats)
-        ctx.meta = (stride, pad, act, is_stem)
+        ctx.save_for_backward(xs, weight, y, stats)
+        ctx.act = act
         ctx.bn_params = (gamma, beta)        # for their .grad (gradient arena): dgamma / dbeta are accumulated in place
         return a
 
     @staticmethod
     def backward(ctx, da):
         xs, weight, y, stats = ctx.saved_tensors
-        stride, pad, act, is_stem = ctx.meta
         Cout = weight.shape[0]
         dab, dacs = _as_nhwc(da, Cout)
         gamma, beta = ctx.bn_params
-        gg, gb = gamma.grad, beta.grad
-        arena = (ACCUMULATE_INTO_GRAD and gg is not None and gb is not None and gg.dtype == torch.float32 and gb.dtype == torch.float32
-                 and gg.is_contiguous() and gb.is_contiguous())
-        dy, dgamma, dbeta = co.bn_backward(dab, y, Cout, stats, act, da_cstride=dacs, dgamma_into=gg if arena else None,
-                                           dbeta_into=gb if arena else None)
-        dx = dw = None
-        # gradient arena: when p.grad already exists (trainer.GradArena) the wgrad is added into it in place and autograd
-        # gets None for the weight (no separate AccumulateGrad add pass, no temporary)
-        tgt = weight.grad if (ACCUMULATE_INTO_GRAD and weight.grad is not None and weight.grad.is_contiguous()) else None
-        side = WGRAD_SIDE["on"] and tgt is not None
-        if is_stem:
-            if side:
-                wgrad_side_run(lambda: co.conv_wgrad(xs, dy, 128, Cout, 1, 1, 0, stem=True, accumulate_into=tgt), (xs, dy))
-            else:
-                dw = co.conv_wgrad(xs, dy, 128, Cout, 1, 1, 0, stem=True, accumulate_into=tgt)
-        else:
-            Cin, k = weight.shape[1], weight.shape[2]
-            N, _, H, W = xs.shape
-            if ctx.needs_input_grad[0]:
-                wd = ctx.wd if ctx.wd is not None else co.pack_weight_dgrad(weight, stride, pad)
-                if ctx.fan is None:
-                    dx = _empty_cl(N, Cin, H, W, da.device)
-                    co.conv_dgrad(dy, wd, N, H, W, Cin, Cout, k, stride, pad, out=_nhwc_of(dx))
-                else:
-                    dx = ctx.fan.add_dgrad(lambda o, ocs, acc: co.conv_dgrad(dy, wd, N, H, W, Cin, Cout, k, stride, pad, out=o,
-                                                                             out_cstride=ocs, accumulate=acc), N, Cin, H, W, da.device)
-            xb, xcs = _as_nhwc(xs, Cin)
-            if side:
-                wgrad_side_run(lambda: co.conv_wgrad(xb, dy, Cin, Cout, k, stride, pad, x_cstride=xcs, accumulate_into=tgt), (xs, xb, dy))
-            else:
-                dw = co.conv_wgrad(xb, dy, Cin, Cout, k, stride, pad, x_cstride=xcs, accumulate_into=tgt)
-        if tgt is not None:
-            dw = None
+        dy, dgamma, dbeta = co.bn_backward(dab, y, Cout, stats, ctx.act, da_cstride=dacs, dgamma_into=_arena_grad(gamma),
+                                           dbeta_into=_arena_grad(beta))
+        dx, dw = _conv_backward(ctx, xs, weight, dy, Cout, ctx.fan)
         dres = None
         if ctx.has_res:
             dres = da if ctx.res_fan is None else ctx.res_fan.put(da)
         return (dx, dw, dgamma, dbeta, None, None, None, None, None, None, None, None, None, None, dres, None, None)
-
-
-class StemFn(torch.autograd.Function):
-    """The 6x6 s2 p2 stem on the raw fp32 NCHW image: im2col (K=108 padded to 128) + pointwise GEMM.  No input grad."""
-
-    @staticmethod
-    def forward(ctx, x, weight):
-        col = co.stem_im2col(x, 1.0)
-        N, H2, W2, _ = col.shape
-        y = _empty_cl(N, weight.shape[0], H2, W2, x.device)
-        co.conv_fwd(col, co.pack_stem_weight(weight), 128, weight.shape[0], 1, 1, 0, None, None, None, out=_nhwc_of(y))
-        ctx.save_for_backward(col)
-        ctx.cout = weight.shape[0]
-        return y
-
-    @staticmethod
-    def backward(ctx, dy):
-        (col,) = ctx.saved_tensors
-        dyb, dycs = _as_nhwc(dy, ctx.cout)
-        dw = co.conv_wgrad(col, dyb, 128, ctx.cout, 1, 1, 0, dy_cstride=dycs, stem=True)
-        return None, dw
-
-
-def _arena_grad(p):
-    """p.grad when it is the contiguous fp32 gradient-arena view the kernels may accumulate into, else None"""
-    g = p.grad
-    return g if (ACCUMULATE_INTO_GRAD and g is not None and g.dtype == torch.float32 and g.is_contiguous()) else None
 
 
 class DetectConvFn(torch.autograd.Function):
@@ -508,9 +484,7 @@ class DetectConvFn(torch.autograd.Function):
         ctx.save_for_backward(x, weight)
         ctx.meta = (na, no)
         ctx.wd, ctx.bias = wd, bias
-        ctx.fan = FanIn.of(x)
-        if ctx.fan is not None:
-            ctx.fan.n += 1
+        ctx.fan = FanIn.join(x)
         return out
 
     @staticmethod
@@ -525,31 +499,15 @@ class DetectConvFn(torch.autograd.Function):
         dyb, partials = co.detect_dy_pack(g, kpad)
         dx = dw = db = None
         if ctx.needs_input_grad[2]:
-            tgt_b = _arena_grad(ctx.bias)
-            db = co.column_sum(partials, out=tgt_b, accumulate=tgt_b is not None)
-            if tgt_b is not None:
-                db = None
+            db = weight_grad(ctx.bias, lambda into: co.column_sum(partials, out=into, accumulate=True))
         if ctx.needs_input_grad[0]:
-            wd = ctx.wd
-            if wd is None:
-                wpad = torch.zeros((kpad, Cin, 1, 1), dtype=torch.float32, device=g.device)
-                wpad[:Cout] = weight.detach().float()
-                wd = co.pack_weight_dgrad(wpad, 1, 0)
-            run = lambda o, ocs, acc: co.conv_dgrad(dyb, wd, N, H, W, Cin, kpad, 1, 1, 0, out=o, out_cstride=ocs, accumulate=acc)  # noqa: E731
-            if ctx.fan is None:
-                dx = _empty_cl(N, Cin, H, W, g.device)
-                run(_nhwc_of(dx), Cin, False)
-            else:
-                dx = ctx.fan.add_dgrad(run, N, Cin, H, W, g.device)
+            wd = ctx.wd if ctx.wd is not None else co.pack_weight_dgrad(weight, 1, 0)    # Cout zero-padded to kpad
+            dx = input_grad(ctx.fan, lambda o, ocs, acc: co.conv_dgrad(dyb, wd, N, H, W, Cin, kpad, 1, 1, 0, out=o, out_cstride=ocs,
+                                                                       accumulate=acc), N, Cin, H, W, g.device)
         if ctx.needs_input_grad[1]:
             xb, xcs = _as_nhwc(x, Cin)
-            tgt = _arena_grad(weight)
-            if WGRAD_SIDE["on"] and tgt is not None:
-                wgrad_side_run(lambda: co.conv_wgrad(xb, dyb, Cin, Cout, 1, 1, 0, x_cstride=xcs, accumulate_into=tgt), (x, xb, dyb))
-            else:
-                dw = co.conv_wgrad(xb, dyb, Cin, Cout, 1, 1, 0, x_cstride=xcs, accumulate_into=tgt)
-            if tgt is not None:
-                dw = None
+            dw = weight_grad(weight, lambda into: co.conv_wgrad(xb, dyb, Cin, Cout, 1, 1, 0, x_cstride=xcs, accumulate_into=into),
+                             (x, xb, dyb))
         return dx, dw, db, None, None, None, None
 
 
@@ -571,9 +529,7 @@ class NetDFn(torch.autograd.Function):
         o = co.netd_tail_fwd(h, C_, w2f)
         ctx.save_for_backward(x, w1, w2, h)
         ctx.wd1n = wd1n
-        ctx.fan = FanIn.of(x)
-        if ctx.fan is not None:
-            ctx.fan.n += 1
+        ctx.fan = FanIn.join(x)
         return o.permute(0, 3, 1, 2)
 
     @staticmethod
@@ -587,31 +543,12 @@ class NetDFn(torch.autograd.Function):
         dh, partials = co.netd_tail_bwd(do, h, C_, w2.detach().float().contiguous())
         dx = dw1 = dw2 = None
         if ctx.needs_input_grad[2]:
-            tgt2 = _arena_grad(w2)
-            if tgt2 is not None:
-                co.column_sum(partials, out=tgt2, accumulate=True)
-            else:
-                dw2 = co.column_sum(partials).view_as(w2)
+            dw2 = weight_grad(w2, lambda into: co.column_sum(partials, out=into, accumulate=True).view_as(w2))
         if ctx.needs_input_grad[0]:
             wd = ctx.wd1n if ctx.wd1n is not None else co.pack_weight_dgrad(-w1.detach().float(), 1, 0)
-            run = lambda o, ocs, acc: co.conv_dgrad(dh, wd, N, H, W, C_, C_, 1, 1, 0, out=o, out_cstride=ocs, accumulate=acc)  # noqa: E731
-            if ctx.fan is None:
-                dx = _empty_cl(N, C_, H, W, g.device)
-                run(_nhwc_of(dx), C_, False)
-            else:
-                dx = ctx.fan.add_dgrad(run, N, C_, H, W, g.device)
+            dx = input_grad(ctx.fan, lambda o, ocs, acc: co.conv_dgrad(dh, wd, N, H, W, C_, C_, 1, 1, 0, out=o, out_cstride=ocs,
+                                                                       accumulate=acc), N, C_, H, W, g.device)
         if ctx.needs_input_grad[1]:
             xb, xcs = _as_nhwc(x, C_)
-            tgt = _arena_grad(w1)
-            if WGRAD_SIDE["on"] and tgt is not None:
-                wgrad_side_run(lambda: co.conv_wgrad(xb, dh, C_, C_, 1, 1, 0, x_cstride=xcs, accumulate_into=tgt), (x, xb, dh))
-            else:
-                dw1 = co.conv_wgrad(xb, dh, C_, C_, 1, 1, 0, x_cstride=xcs, accumulate_into=tgt)
-            if tgt is not None:
-                dw1 = None
+            dw1 = weight_grad(w1, lambda into: co.conv_wgrad(xb, dh, C_, C_, 1, 1, 0, x_cstride=xcs, accumulate_into=into), (x, xb, dh))
         return dx, dw1, dw2, None, None
-
-
-def conv2d_native(x, weight, stride, pad):
-    _lib.require_cuda(x, weight)
-    return ConvFn.apply(x, weight, stride, pad)

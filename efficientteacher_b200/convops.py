@@ -69,6 +69,11 @@ def stem_im2col(x_nchw_f32, mul=1.0):
     return out
 
 
+def _conv_params(N, H, W, Cin, Cout, k, stride, pad, **fields):
+    """EtbConvParams of a k x k convolution; `fields` sets the remaining members (pixel strides, offsets, act, det_no)"""
+    return EtbConvParams(N=N, H=H, W=W, Cin=Cin, Cout=Cout, kh=k, kw=k, stride=stride, pad=pad, **fields)
+
+
 def conv_fwd(x, w_packed, Cin, Cout, k, stride, pad, scale=None, bias=None, act="silu", out=None, out_coffset=0,
              x_coffset=0, residual=None, res_coffset=0, det_out=None, det_no=0, x_cstride=None):
     """x: [N,H,W,Cs] bf16 NHWC (logical channels [x_coffset, x_coffset+Cin)).  Returns `out` (bf16 NHWC, written at
@@ -79,13 +84,7 @@ def conv_fwd(x, w_packed, Cin, Cout, k, stride, pad, scale=None, bias=None, act=
         cs = x_cstride
     Ho = (H + 2 * pad - k) // stride + 1
     Wo = (W + 2 * pad - k) // stride + 1
-    cp = EtbConvParams()
-    cp.N, cp.H, cp.W, cp.Cin, cp.Cout = N, H, W, Cin, Cout
-    cp.kh = cp.kw = k
-    cp.stride, cp.pad = stride, pad
-    cp.x_cstride = cs
-    cp.act = ACT[act]
-    cp.det_no = det_no
+    cp = _conv_params(N, H, W, Cin, Cout, k, stride, pad, x_cstride=cs, act=ACT[act], det_no=det_no)
     xp = x.data_ptr() + 2 * x_coffset
     if det_out is None:
         if out is None:
@@ -106,8 +105,10 @@ def sppf_pool(buf, Cq):
     return buf
 
 
-def upsample2x(x, Cc, out, out_coffset, x_coffset=0):
+def upsample2x(x, Cc, out, out_coffset, x_coffset=0, x_cstride=None):
     N, H, W, cs = x.shape
+    if x_cstride is not None:     # x is a strided channel-slice view: pixel stride given explicitly
+        cs = x_cstride
     _lib.check(_lib.lib().etb_upsample2x_nhwc(_lib.ptr(x), _lib.ptr(out), N, H, W, Cc, cs, x_coffset, out.shape[3], out_coffset,
                                               _lib.stream_ptr()), "etb_upsample2x_nhwc")
     return out
@@ -127,14 +128,10 @@ def conv_dgrad(dy, wd_packed, N, H, W, Cin, Cout, k, stride, pad, out=None, out_
                dy_cstride=None, out_cstride=None):
     """dy: [N,Ho,Wo,Cs] bf16 NHWC (channels [dy_coffset, +Cout)) -> dx [N,H,W,*] bf16 at channel offset out_coffset."""
     _lib.require_cuda(dy, wd_packed)
-    cp = EtbConvParams()
-    cp.N, cp.H, cp.W, cp.Cin, cp.Cout = N, H, W, Cin, Cout
-    cp.kh = cp.kw = k
-    cp.stride, cp.pad = stride, pad
-    cp.x_cstride = dy.shape[3] if dy_cstride is None else dy_cstride
     if out is None:
         out = nhwc_empty(N, H, W, Cin, dy.device)
-    cp.y_cstride, cp.y_coffset = (out.shape[3] if out_cstride is None else out_cstride), out_coffset
+    cp = _conv_params(N, H, W, Cin, Cout, k, stride, pad, x_cstride=dy.shape[3] if dy_cstride is None else dy_cstride,
+                      y_cstride=out.shape[3] if out_cstride is None else out_cstride, y_coffset=out_coffset)
     _lib.check(_lib.lib().etb_conv_dgrad(C.c_void_p(dy.data_ptr() + 2 * dy_coffset), _lib.ptr(wd_packed), _lib.ptr(out), C.byref(cp),
                                          int(accumulate), _lib.stream_ptr()), "etb_conv_dgrad")
     return out
@@ -147,12 +144,8 @@ def conv_wgrad(x, dy, Cin, Cout, k, stride, pad, x_coffset=0, dy_coffset=0, stem
     returned (saves the separate AccumulateGrad pass)."""
     _lib.require_cuda(x, dy)
     N, H, W, xcs = x.shape
-    cp = EtbConvParams()
-    cp.N, cp.H, cp.W, cp.Cin, cp.Cout = N, H, W, Cin, Cout
-    cp.kh = cp.kw = k
-    cp.stride, cp.pad = stride, pad
-    cp.x_cstride = xcs if x_cstride is None else x_cstride
-    cp.y_cstride = dy.shape[3] if dy_cstride is None else dy_cstride
+    cp = _conv_params(N, H, W, Cin, Cout, k, stride, pad, x_cstride=xcs if x_cstride is None else x_cstride,
+                      y_cstride=dy.shape[3] if dy_cstride is None else dy_cstride)
     lib = _lib.lib()
     xp, dyp = C.c_void_p(x.data_ptr() + 2 * x_coffset), C.c_void_p(dy.data_ptr() + 2 * dy_coffset)
     acc = accumulate_into

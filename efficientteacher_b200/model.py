@@ -76,23 +76,18 @@ class Conv(nn.Module):
         """res: shortcut added after the activation; dest/coff: autograd_conv.CatBuf slice to write the output into
         (both only on the fused path -- callers check `glue(x)` first)."""
         if Conv.NATIVE and x.is_cuda:
-            from .autograd_conv import ConvBnActFn, ConvFn, StemFn
-            w = self.conv.weight
+            from .autograd_conv import ConvBnActFn, ConvFn
+            w, s, p = self.conv.weight, self.conv.stride[0], self.conv.padding[0]
+            # operands prepared by Model.pack_weights() (one launch per training step)
+            pc = getattr(self, "_packed", None) if Conv.FUSED_BN and self.training else None
+            wp, wd = (None, None) if pc is None else (pc.fwd, pc.dgrad)
             if self.fused(x):
                 bn = self.bn
                 act = "silu" if isinstance(self.act, nn.SiLU) else "relu"
-                pc = getattr(self, "_packed", None)     # operands prepared by Model.pack_weights() (one launch per step)
-                return ConvBnActFn.apply(x, w, bn.weight, bn.bias, bn.running_mean, bn.running_var, self.conv.stride[0],
-                                         self.conv.padding[0], bn.eps, bn.momentum, act, self.is_stem,
-                                         None if pc is None else pc.fwd, None if pc is None else pc.dgrad, res, dest, coff)
+                return ConvBnActFn.apply(x, w, bn.weight, bn.bias, bn.running_mean, bn.running_var, s, p, bn.eps, bn.momentum, act,
+                                         self.is_stem, wp, wd, res, dest, coff)
             assert dest is None
-            if self.is_stem:
-                if not torch.is_tensor(x):          # autograd_conv.StemInput on the scaffold path: materialise the batch
-                    x = torch.cat([q.float() for q in x.parts], 0) / x.div
-                y = StemFn.apply(x.float(), w)
-            else:
-                y = ConvFn.apply(x, w, self.conv.stride[0], self.conv.padding[0])
-            y = self.act(self.bn(y))
+            y = self.act(self.bn(ConvFn.apply(x, w, s, p, self.is_stem, wp, wd)))
             return y if res is None else res + y
         assert dest is None
         y = self.act(self.bn(self.conv(x)))
@@ -390,7 +385,7 @@ class _ModelBase(nn.Module):
         tensors to be concatenated along the batch (the loaders' raw batches: trainer/ssod_trainer.py:620,694-696).  On the
         native path this becomes an autograd_conv.StemInput (no cat, no fp32 image); otherwise a plain fp32 tensor."""
         parts = list(x) if isinstance(x, (list, tuple)) else [x]
-        native = Conv.NATIVE and Conv.FUSED_BN and self.training and all(p.is_cuda for p in parts)
+        native = Conv.NATIVE and self.training and all(p.is_cuda for p in parts)
         if native and (len(parts) > 1 or parts[0].dtype == torch.uint8):
             from .autograd_conv import StemInput
             return StemInput(parts)

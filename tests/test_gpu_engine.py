@@ -100,7 +100,7 @@ def test_native_training_convs_vs_fp32_reference():
     At random init with a tiny batch the parameter gradients of ANY bf16 implementation only correlate ~0.8 with fp32
     (tools/debug_grad_noise.py: native 0.81, torch/cuDNN bf16 0.77), so the criterion is: against an fp32 (TF32 off) torch
     reference of the same step the native path is at least as accurate as the library bf16 path, per parameter; the
-    per-kernel tolerance tests live in test_gpu_conv.py and tools/debug_train_convs.py checks every layer in situ."""
+    per-kernel tolerance tests live in test_gpu_conv.py and test_gpu_geometry.py."""
     from efficientteacher_b200 import model as M
     from efficientteacher_b200.config import yolov5_ssod_cfg
     from efficientteacher_b200.loss import ComputeLoss
