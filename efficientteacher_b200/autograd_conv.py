@@ -174,6 +174,21 @@ def split_batch(t, n):
     return a, b
 
 
+class ZeroTermFn(torch.autograd.Function):
+    """0 * (t_0.mean() + t_1.mean() + ...) for finite t_i (trainer/ssod_trainer.py:516 keeps the unlabeled Detect outputs in
+    the graph that way): value 0, gradient exact zeros.  The zeros are written into each tensor's grad_buffer_for
+    destination, so a batch half that came out of split_batch keeps SplitBatchFn's zero-copy backward."""
+
+    @staticmethod
+    def forward(ctx, *ts):
+        ctx.ts = ts          # the tensors themselves: grad_buffer_for reads their split_batch tag
+        return torch.zeros(1, dtype=torch.float32, device=ts[0].device)
+
+    @staticmethod
+    def backward(ctx, g):
+        return tuple(grad_buffer_for(t).zero_() for t in ctx.ts)
+
+
 class CatBuf:
     """A concat buffer [N, Ct, H, W] (channels_last = NHWC in memory).  Producers write their outputs straight into
     channel slices of `buf` (concat-by-offset, the training-side twin of engine.TrunkEngine's layout) and JoinFn turns

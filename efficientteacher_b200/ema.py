@@ -87,14 +87,15 @@ def _launch(table, d, d2=0.0, scalars_dev=None):
 
 
 class _EMABase:
-    def _update_with(self, model, d):
+    def _update_with(self, model, d, scalars_dev=None):
+        """scalars_dev: ema_scalars(d) in device memory (graph capture: the decay is refreshed before each replay)"""
         with torch.no_grad():
             v_list, m_list = _float_pairs(self.ema, model)
             key = tuple(t.data_ptr() for t in v_list) + tuple(t.data_ptr() for t in m_list)
             tab = getattr(self, "_table", None)
             if tab is None or tab.key != key:
                 tab = self._table = _ChunkTable(v_list, m_list)
-            _launch(tab, d)
+            _launch(tab, d, scalars_dev=scalars_dev)
 
     def update_attr(self, model, include=(), exclude=('process_group', 'reducer')):
         copy_attr(self.ema, model, include, exclude)

@@ -120,15 +120,20 @@ class ComputeLoss:
         self.assigner = YOLOAnchorAssigner(self.na, self.nl, self.anchors, self.anchor_t, det.stride, self.nc,
                                            self.num_keypoints, single_targets=self.single_targets, ota=False)
 
-    def default_loss(self, p, targets):
+    def default_loss(self, p, targets, n_dev=None):
+        """n_dev (int32[1] CUDA): targets is a buffer of capacity targets.shape[0] whose first n_dev rows are the labels --
+        the label count stays on the device, so one captured graph serves batches with any number of labels."""
         p = _prep_p(p)
         targets = targets.to(p[0].device)
-        sets = [self.assigner.assign(p, targets)]
+        if n_dev is None:
+            sets = [self.assigner.assign(p, targets)]
+        else:
+            sets = [self.assigner.assign(p, targets, nt_dev=n_dev, cap_rows=targets.shape[0])]
         lp = make_loss_params(p, self.na, self.balance, self.box_w, self.obj_w, self.cls_w, self.cp, self.cn)
         out4 = _FusedDetLoss.apply(lp, sets, "sup", *p)
         lbox, lobj, lcls = out4[0:1].detach(), out4[1:2].detach(), out4[2:3].detach()
         loss = out4[3:4]
         return loss, dict(box=lbox, obj=lobj, cls=lcls, loss=loss)
 
-    def __call__(self, p, targets):
-        return self.default_loss(p, targets)
+    def __call__(self, p, targets, n_dev=None):
+        return self.default_loss(p, targets, n_dev)

@@ -87,6 +87,8 @@ class SSODTrainerStep:
         self._teacher_stream = None
         self._teacher_keep = None
         self._bn_sync = None
+        self._burn_graph = None     # captured burn-in step (train_without_unlabeled[_da]_graphed)
+        self.burn_in_captures = 0   # how many times a burn-in step has been captured
 
     # trainer/trainer.py:193-217
     def build_optimizer(self, cfg):
@@ -207,6 +209,7 @@ class SSODTrainerStep:
     # trainer/ssod_trainer.py:587-680 (logging / meters excluded: rank-0 host bookkeeping)
     def train_instance(self, imgs, targets, unlabeled_imgs, unlabeled_imgs_ori, unlabeled_gt, unlabeled_M, ni,
                        host_pseudo_labels=False, _stop_after_backward=False):
+        self._require_semi_ema()
         n_img = imgs.shape[0]
         self._mark("start")
         if self.WORLD_SIZE > 1 and not torch.cuda.is_current_stream_capturing():
@@ -290,8 +293,7 @@ class SSODTrainerStep:
         ~1.5k kernel launches + the autograd traversal collapse into two cudaGraphLaunch calls.  Inputs are copied into
         static buffers; learning rate / momentum (warm-up, scheduler) and the EMA decays of the step are host scalars
         written to device memory before B is replayed, so the schedule needs no re-capture."""
-        if self.semi_ema is None:
-            raise NotImplementedError("graphed step needs the fused ema/semi_ema pair (burn_epochs == 0)")
+        self._require_semi_ema()
         shapes = (tuple(imgs.shape), tuple(targets.shape), tuple(unlabeled_imgs.shape), tuple(unlabeled_M.shape),
                   imgs.dtype, unlabeled_imgs.dtype, unlabeled_imgs_ori.dtype)      # uint8 loader batches vs fp32: different static buffers
         if self._graph is not None and self._graph["shapes"] != shapes:
@@ -345,17 +347,7 @@ class SSODTrainerStep:
         self._ema_scalars_dev = torch.zeros(4, dtype=torch.float32, device=dev)
         was_profile, self.profile = self.profile, False
         self.last = {}
-        # the warm-up steps below really train: snapshot every piece of state they touch and restore it afterwards
-        self._ensure_arena()
-        had_momentum = any(len(self.optimizer.state[p]) for g_ in self.optimizer.param_groups for p in g_["params"])
-        tensors = [t for m in (self.model, self.ema.ema, self.semi_ema.ema) for t in m.state_dict().values()]
-        if had_momentum:
-            tensors += [self.optimizer.state[p]["momentum_buffer"] for g_ in self.optimizer.param_groups for p in g_["params"]
-                        if self.optimizer.state[p].get("momentum_buffer") is not None]
-        tensors.append(self._arena.flat)     # gradients already accumulated towards the next optimizer step (accumulate > 1)
-        snap = [t.clone() for t in tensors]
-        saved = (self.last_opt_step, self.ema.updates, self.semi_ema.updates, self.accumulate,
-                 [(x['lr'], x.get('momentum')) for x in self.optimizer.param_groups])
+        restore = self._snapshot_training_state()
         lm_state = None
         if hasattr(self.pseudo_label_creator, "count"):
             lm_state = (self.pseudo_label_creator.count, self.pseudo_label_creator.pse_count)
@@ -378,24 +370,200 @@ class SSODTrainerStep:
         with torch.cuda.graph(gb, pool=graph.pool()):
             self._step_and_ema(capturing=True)
         st["graph_b"] = gb
-        with torch.no_grad():
-            for t, c in zip(tensors, snap):
-                t.copy_(c)
-            if not had_momentum:      # buffers created by the warm-up: zero == "not yet created" for SGD (buf = grad on first use)
-                for g_ in self.optimizer.param_groups:
-                    for p in g_["params"]:
-                        b = self.optimizer.state[p].get("momentum_buffer")
-                        if b is not None:
-                            b.zero_()
-        self.last_opt_step, self.ema.updates, self.semi_ema.updates, self.accumulate, hyp = saved
-        for x, (lr, mom) in zip(self.optimizer.param_groups, hyp):
-            x['lr'] = lr
-            if mom is not None:
-                x['momentum'] = mom
+        restore()
         if lm_state is not None:
             self.pseudo_label_creator.count, self.pseudo_label_creator.pse_count = lm_state
         self.profile = was_profile
         self._graph = st
+
+    def _snapshot_training_state(self):
+        """The warm-up steps before a capture really train: snapshot every piece of state they touch (weights, BN
+        statistics, the EMA model(s), momentum, the gradients accumulated towards the next optimizer step, the counters,
+        lr / momentum) and return the function that puts it back."""
+        self._ensure_arena()
+        emas = [e for e in (self.ema, self.semi_ema) if e is not None]
+        had_momentum = any(len(self.optimizer.state[p]) for g_ in self.optimizer.param_groups for p in g_["params"])
+        tensors = [t for m in [self.model] + [e.ema for e in emas] for t in m.state_dict().values()]
+        if had_momentum:
+            tensors += [self.optimizer.state[p]["momentum_buffer"] for g_ in self.optimizer.param_groups for p in g_["params"]
+                        if self.optimizer.state[p].get("momentum_buffer") is not None]
+        tensors.append(self._arena.flat)     # gradients already accumulated towards the next optimizer step (accumulate > 1)
+        snap = [t.clone() for t in tensors]
+        saved = (self.last_opt_step, [e.updates for e in emas], self.accumulate,
+                 [(x['lr'], x.get('momentum')) for x in self.optimizer.param_groups])
+
+        def restore():
+            with torch.no_grad():
+                for t, c in zip(tensors, snap):
+                    t.copy_(c)
+                if not had_momentum:      # buffers created by the warm-up: zero == "not yet created" for SGD (buf = grad on first use)
+                    for g_ in self.optimizer.param_groups:
+                        for p in g_["params"]:
+                            b = self.optimizer.state[p].get("momentum_buffer")
+                            if b is not None:
+                                b.zero_()
+            self.last_opt_step, updates, self.accumulate, hyp = saved
+            for e, u in zip(emas, updates):
+                e.updates = u
+            for x, (lr, mom) in zip(self.optimizer.param_groups, hyp):
+                x['lr'] = lr
+                if mom is not None:
+                    x['momentum'] = mom
+        return restore
+
+    # ---- burn-in: trainer/ssod_trainer.py:295-317 (train_in_epoch), :421-456 / :490-533 -----------------------------
+    @property
+    def in_burn_in(self):
+        """True while epoch < hyp.burn_epochs: the step is train_without_unlabeled[_da] (labeled data only, or + the weak
+        unlabeled images with the domain losses), with ONE ModelEMA and no semi_ema."""
+        return self.epoch < self.cfg.hyp.burn_epochs
+
+    def _require_semi_ema(self):
+        if self.semi_ema is None:
+            raise RuntimeError("the semi-supervised step needs semi_ema, which begin_epoch(epoch) creates at epoch == "
+                               "hyp.burn_epochs (%d); current epoch %d%s" % (
+                                   self.cfg.hyp.burn_epochs, self.epoch,
+                                   ": still in burn-in, use train_without_unlabeled[_da]" if self.in_burn_in else
+                                   " is past it (a run resumed after burn-in never gets a semi_ema, as in the reference)"))
+
+    def begin_epoch(self, epoch):
+        """The trainer's side of ssod_trainer.py:295-317: sets the epoch; at epoch == burn_epochs (> 0) the semi-supervised
+        EMA is created from the burn-in EMA and the burn-in graphs are dropped, so train_instance[_graphed] runs from here on.
+        The reference's loop that 'copies the EMA into the student' (:306-309) only assigns into a temporary state_dict()
+        dict, so it changes nothing: the student is deliberately NOT reset to the EMA here either."""
+        self.epoch = epoch
+        burn = self.cfg.hyp.burn_epochs
+        if burn > 0 and epoch == burn:
+            if self.cfg.SSOD.cosine_ema:
+                self.semi_ema = CosineEMA(self.ema.ema, decay_start=self.cfg.SSOD.ema_rate, total_epoch=self.epochs - burn)
+            else:
+                self.semi_ema = SemiSupModelEMA(self.ema.ema, self.cfg.SSOD.ema_rate)
+            self._burn_graph = None
+
+    def _burn_in_loss(self, imgs, targets, unlabeled_imgs_ori=None, n_dev=None):
+        """Forward + loss of the burn-in step (the reference computes it under autocast; the fused loss kernels read fp32).
+        unlabeled_imgs_ori=None: train_without_unlabeled (:427-443), else train_without_unlabeled_da (:498-520)."""
+        if self.WORLD_SIZE > 1 and not torch.cuda.is_current_stream_capturing():
+            self._bn_broadcast()         # (captured steps: _burn_in_graphed issues it before the replay)
+        with torch.autocast("cuda", dtype=self.amp_dtype):
+            # the native stem reads uint8 or fp32 batches in place; with two batches the cat is never materialised
+            pred, feats = self.model(imgs if unlabeled_imgs_ori is None else [imgs, unlabeled_imgs_ori])
+        if unlabeled_imgs_ori is None:
+            loss, items = self.compute_loss(pred, targets, n_dev)
+            # netD stays in the graph with zero gradients, so SGD still applies weight decay + momentum to its weights
+            loss = loss + 0 * (feats[0].mean() + feats[1].mean() + feats[2].mean())
+        else:
+            sup_pred, sup_feature, un_sup_pred, un_sup_feature = self.split_predict_and_feature(pred, feats, imgs.shape[0])
+            loss, items = self.compute_loss(sup_pred, targets, n_dev)
+            w = self.da_loss_weights
+            from .autograd_conv import ZeroTermFn
+            # + 0 * un_sup_pred[i].mean(): the unlabeled half of the Detect gradient is zero-filled in place
+            loss = loss + self.domain_loss(sup_feature) * w + self.target_loss(un_sup_feature) * w + ZeroTermFn.apply(*un_sup_pred)
+        return loss, items
+
+    def _burn_in_step(self, imgs, targets, unlabeled_imgs_ori, ni):
+        loss, items = self._burn_in_loss(imgs, targets, unlabeled_imgs_ori)
+        self.update_optimizer(loss, ni)
+        self.last = dict(loss=loss.detach(), sup={k: v.detach() for k, v in items.items()})
+        return loss.detach()
+
+    def train_without_unlabeled(self, imgs, targets, ni):
+        """ssod_trainer.py:421-456, one iteration: labeled images only; backward, warm-up / accumulate, SGD, ema.update"""
+        return self._burn_in_step(imgs, targets, None, ni)
+
+    def train_without_unlabeled_da(self, imgs, targets, unlabeled_imgs_ori, ni):
+        """ssod_trainer.py:490-533, one iteration: labeled + weak unlabeled images, detection loss on the labeled half plus
+        the domain losses (SSOD.da_loss_weights) of both halves"""
+        return self._burn_in_step(imgs, targets, unlabeled_imgs_ori, ni)
+
+    def train_without_unlabeled_graphed(self, imgs, targets, ni):
+        """train_without_unlabeled replayed from captured CUDA graphs; see _burn_in_graphed"""
+        return self._burn_in_graphed(imgs, targets, None, ni)
+
+    def train_without_unlabeled_da_graphed(self, imgs, targets, unlabeled_imgs_ori, ni):
+        """train_without_unlabeled_da replayed from captured CUDA graphs; see _burn_in_graphed"""
+        return self._burn_in_graphed(imgs, targets, unlabeled_imgs_ori, ni)
+
+    BURN_IN_LABEL_CAPACITY = 64       # initial label capacity of a burn-in graph; doubles when a batch has more labels
+
+    def _burn_in_graphed(self, imgs, targets, uw, ni):
+        """The burn-in step as two graphs, like train_instance_graphed: A = forward + loss + backward, [all-reduce], B =
+        SGD-Nesterov + the single EMA update with its decay read from device memory.  The labels are copied into a static
+        buffer of capacity C and their count into a device int32 (stream-ordered, no host sync) that the assigner reads,
+        so one capture serves every batch of a given image shape and dtype whatever its label count; a batch with more
+        than C labels re-captures with C doubled until it fits."""
+        if self.semi_ema is not None:
+            raise RuntimeError("burn-in step requested after the hand-over to the semi-supervised phase (semi_ema exists)")
+        nt = int(targets.shape[0])
+        key = (tuple(imgs.shape), imgs.dtype, None if uw is None else (tuple(uw.shape), uw.dtype))
+        g = self._burn_graph
+        cap = self.BURN_IN_LABEL_CAPACITY if g is None else g["cap"]
+        while cap < nt:
+            cap *= 2
+        if g is None or g["key"] != key or g["cap"] != cap:
+            self._burn_graph = None
+            g = self._capture_burn_in(imgs, targets, uw, ni, key, cap)
+        g["imgs"].copy_(imgs, non_blocking=True)
+        if uw is not None:
+            g["uw"].copy_(uw, non_blocking=True)
+        g["targets"][:nt].copy_(targets, non_blocking=True)
+        # pageable sources: the runtime stages these few bytes before returning, so the next step cannot overwrite them early
+        g["nt"].copy_(torch.tensor([nt], dtype=torch.int32))
+        due = self._warmup(ni)
+        if due:
+            self.ema.updates += 1
+            g["ema_dev"].copy_(torch.tensor(ema_scalars(self.ema.decay(self.ema.updates)), dtype=torch.float32))
+            self.optimizer.refresh_hyper()
+        self._bn_broadcast()
+        g["graph"].replay()
+        if due:
+            self._allreduce_grads()
+            g["graph_b"].replay()
+            self.last_opt_step = ni
+        return g["loss"]
+
+    def _burn_in_forward_backward(self, st):
+        # returns the loss detached: nothing may keep this step's autograd graph alive, because the AccumulateGrad nodes of
+        # the parameters it holds are tied to the stream they were created on (the warm-up's side stream, the capture's)
+        loss, _ = self._burn_in_loss(st["imgs"], st["targets"], st["uw"], st["nt"])
+        self._backward(loss)
+        return loss.detach()
+
+    def _capture_burn_in(self, imgs, targets, uw, ni, key, cap):
+        dev = self.device
+        nt = int(targets.shape[0])
+        st = dict(key=key, cap=cap, imgs=imgs.clone(), uw=None if uw is None else uw.clone(),
+                  targets=torch.zeros((cap, 6), dtype=torch.float32, device=dev),
+                  nt=torch.full((1,), nt, dtype=torch.int32, device=dev),
+                  ema_dev=torch.zeros(4, dtype=torch.float32, device=dev))
+        st["targets"][:nt].copy_(targets)
+        was_profile, self.profile = self.profile, False
+        self.last = {}
+        restore = self._snapshot_training_state()
+        side = torch.cuda.Stream(device=dev)
+        side.wait_stream(torch.cuda.current_stream(dev))
+        with torch.cuda.stream(side):
+            for _ in range(2):
+                self._burn_in_forward_backward(st)
+                self._allreduce_grads()
+                self._warmup(ni)
+                self._step_and_ema()
+        torch.cuda.current_stream(dev).wait_stream(side)
+        torch.cuda.synchronize(dev)
+        graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(graph):
+            st["loss"] = self._burn_in_forward_backward(st)
+        st["graph"] = graph
+        gb = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(gb, pool=graph.pool()):
+            self.optimizer.step(zero_grad=True)
+            self.ema._update_with(self.model, 0.0, scalars_dev=st["ema_dev"])
+        st["graph_b"] = gb
+        restore()
+        self.profile = was_profile
+        self.burn_in_captures += 1
+        self._burn_graph = st
+        return st
 
 
 class SupTrainerStep:
