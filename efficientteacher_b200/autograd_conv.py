@@ -438,7 +438,7 @@ class ConvFn(torch.autograd.Function):
 
 class ConvBnActFn(torch.autograd.Function):
     """a = act(BatchNorm_train(conv2d(x, w))) -- the whole Conv module (common.py:480-481) in training mode:
-    wgmma conv -> per-channel batch statistics -> fused normalise+SiLU; backward = fused SiLU'/BN backward (2 passes)
+    wgmma conv -> per-channel batch statistics -> fused normalise+activation; backward = fused act'/BN backward (2 passes)
     -> dgrad + wgrad.  Saves x, the raw conv output and [4,C] statistics (not the normalised tensor)."""
 
     @staticmethod

@@ -8,11 +8,11 @@ COCO_NAMES = [str(i) for i in range(80)]
 ANCHORS = [[10, 13, 16, 30, 33, 23], [30, 61, 62, 45, 59, 119], [116, 90, 156, 198, 373, 326]]
 
 
-def _model(depth, width):
+def _model(depth, width, backbone_act='SiLU', neck_act='SiLU'):
     return NS(depth_multiple=depth, width_multiple=width, ch=3, inplace=True, anchors=[list(a) for a in ANCHORS],
               RepOpt=False, weights='',
-              Backbone=NS(name='YoloV5', activation='SiLU'),
-              Neck=NS(name='YoloV5', activation='SiLU', in_channels=[256, 512, 1024], out_channels=[256, 512, 1024]),
+              Backbone=NS(name='YoloV5', activation=backbone_act),
+              Neck=NS(name='YoloV5', activation=neck_act, in_channels=[256, 512, 1024], out_channels=[256, 512, 1024]),
               Head=NS(name='YoloV5', activation='SiLU', strides=[8, 16, 32]))
 
 
@@ -36,15 +36,17 @@ def _ssod():
               extra_teachers=[], multi_step_lr=False)
 
 
-def yolov5_ssod_cfg(size='l', batch_size=32, img_size=640):
+def yolov5_ssod_cfg(size='l', batch_size=32, img_size=640, backbone_act='SiLU', neck_act='SiLU'):
+    """backbone_act / neck_act: cfg.Model.{Backbone,Neck}.activation -- 'SiLU', 'ReLU', or anything else for the Hardswish
+    trunk (the reference's defaults, configs/defaults.py, are 'LeakyReLU' and 'ReLU': a Hardswish backbone, a ReLU neck)"""
     depth, width = {'l': (1.0, 1.0), 's': (0.33, 0.50), 'm': (0.67, 0.75), 'l_shallow': (0.33, 1.0)}[size]
     return NS(epochs=300, adam=False, linear_lr=True, single_cls=False, sync_bn=False,
-              hyp=_hyp(), Model=_model(depth, width), Loss=_loss(), SSOD=_ssod(),
+              hyp=_hyp(), Model=_model(depth, width, backbone_act, neck_act), Loss=_loss(), SSOD=_ssod(),
               Dataset=NS(nc=80, np=0, names=list(COCO_NAMES), img_size=img_size, batch_size=batch_size))
 
 
-def yolov5_sup_cfg(size='l', batch_size=32, img_size=640):
-    cfg = yolov5_ssod_cfg(size, batch_size, img_size)
+def yolov5_sup_cfg(size='l', batch_size=32, img_size=640, backbone_act='SiLU', neck_act='SiLU'):
+    cfg = yolov5_ssod_cfg(size, batch_size, img_size, backbone_act, neck_act)
     cfg.SSOD.train_domain = False
     cfg.linear_lr = False
     return cfg

@@ -6,7 +6,8 @@ import torch
 from . import _lib
 from ._lib import EtbConvParams
 
-ACT = {None: 0, "none": 0, "silu": 1, "relu": 2}
+# activation codes of the conv epilogue and the BatchNorm kernels (include/etb200.h); 3 is not a code
+ACT = {None: 0, "none": 0, "silu": 1, "relu": 2, "hard_swish": 4}
 
 
 def nhwc_empty(N, H, W, C, device):

@@ -1,4 +1,4 @@
-// bn.cu -- training-mode BatchNorm2d + SiLU around the wgmma convolutions, forward and backward (K1/K2 tails).
+// bn.cu -- training-mode BatchNorm2d + SiLU / ReLU / Hardswish around the wgmma convolutions, forward and backward (K1/K2 tails).
 //   Conv.forward = act(bn(conv(x)))           reference models/backbone/common.py:480-481
 //   BN settings eps=1e-3, momentum=0.03       reference utils/torch_utils.py:162-171 (initialize_weights)
 // Replaces, per Conv, ATen's batch_norm_collect_statistics + batch_norm_transform_input + SiLU (5 passes over the
@@ -185,10 +185,22 @@ __device__ __forceinline__ float dsilu_f(float z) {
   return s * fmaf(z, 1.0f - s, 1.0f);
 }
 
+// act(z) / act'(z).  HSWISH selects the Hardswish instance of each kernel (act 4); the other instance reads act 0 / 1 / 2 at
+// run time.  Hardswish as a third run-time case would cost the SiLU kernels registers (bn_act_bwd_apply 114 -> 128).
+template <bool HSWISH>
+__device__ __forceinline__ float bn_act(float z, int act) {
+  return HSWISH ? hswish_f(z) : (act == 1 ? silu_f(z) : (act == 2 ? fmaxf(z, 0.f) : z));
+}
+template <bool HSWISH>
+__device__ __forceinline__ float bn_dact(float z, int act) {   // ReLU'(0) = 0, as threshold_backward takes it
+  return HSWISH ? dhswish_f(z) : (act == 1 ? dsilu_f(z) : (act == 2 ? (z > 0.f ? 1.f : 0.f) : 1.f));
+}
+
 // ---- forward apply: a = act(y*scale + shift) ----
 // The grid stride (gridDim.x*256 vectors) is a multiple of G = C/8 (a power of two <= 256), so a thread's channel group
 // never changes: its scale/shift live in registers for the whole kernel and the loop body is 2 independent 16 B loads,
 // 8 FMAs + SiLU, 2 stores.
+template <bool HSWISH>
 __global__ void __launch_bounds__(BN_THREADS) bn_act_apply_kernel(const __nv_bfloat16* __restrict__ y, const float* __restrict__ scale,
                                                                   const float* __restrict__ shift, __nv_bfloat16* __restrict__ out, long M, int C,
                                                                   int ycs, int ocs, int act, const __nv_bfloat16* __restrict__ res, int rcs) {
@@ -207,7 +219,7 @@ __global__ void __launch_bounds__(BN_THREADS) bn_act_apply_kernel(const __nv_bfl
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
       const float z = fmaf(f[j], sc[j], sh[j]);
-      f[j] = act == 1 ? silu_f(z) : (act == 2 ? fmaxf(z, 0.f) : z);
+      f[j] = bn_act<HSWISH>(z, act);
     }
     if (res) {      // Bottleneck shortcut (common.py:499): x + cv2(cv1(x)); the sum is rounded once, from fp32
       float q[8];
@@ -243,6 +255,7 @@ __global__ void __launch_bounds__(BN_THREADS) bn_act_apply_kernel(const __nv_bfl
 }
 
 // ---- backward reduce: sums[0][c] = sum dz, sums[1][c] = sum dz*xhat,  dz = da * act'(z) ----
+template <bool HSWISH>
 __global__ void __launch_bounds__(BN_THREADS) bn_act_bwd_reduce_kernel(const __nv_bfloat16* __restrict__ da, const __nv_bfloat16* __restrict__ y,
                                                                        const float* __restrict__ scale, const float* __restrict__ shift,
                                                                        const float* __restrict__ mean, const float* __restrict__ invstd, int M,
@@ -267,7 +280,7 @@ __global__ void __launch_bounds__(BN_THREADS) bn_act_bwd_reduce_kernel(const __n
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
       const float z = fmaf(fy[j], sc[j], sh[j]);
-      const float dz = fd[j] * (act == 1 ? dsilu_f(z) : (act == 2 ? (z > 0.f ? 1.f : 0.f) : 1.f));
+      const float dz = fd[j] * bn_dact<HSWISH>(z, act);
       const float xh = fmaf(fy[j], is[j], mu[j]);
       acc[0][j] += dz;
       acc[1][j] = fmaf(dz, xh, acc[1][j]);
@@ -297,6 +310,7 @@ __global__ void __launch_bounds__(BNR_CH * BNR_GR) bn_bwd_finalize_kernel(const 
 // ---- backward apply: dy = gamma*invstd * (dz - sum_dz/M - xhat*sum_dz_xhat/M) ----
 // Same fixed-channel-group structure as the forward apply: the six per-channel vectors are folded into five register
 // arrays once per thread.
+template <bool HSWISH>
 __global__ void __launch_bounds__(BN_THREADS, 2) bn_act_bwd_apply_kernel(const __nv_bfloat16* __restrict__ da, const __nv_bfloat16* __restrict__ y,
                                                                       const float* __restrict__ scale, const float* __restrict__ shift,
                                                                       const float* __restrict__ mean, const float* __restrict__ invstd,
@@ -330,7 +344,7 @@ __global__ void __launch_bounds__(BN_THREADS, 2) bn_act_bwd_apply_kernel(const _
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
       const float z = fmaf(fy[j], sc[j], sh[j]);
-      const float dz = fd[j] * (act == 1 ? dsilu_f(z) : (act == 2 ? (z > 0.f ? 1.f : 0.f) : 1.f));
+      const float dz = fd[j] * bn_dact<HSWISH>(z, act);
       fd[j] = fmaf(sc[j], dz, fmaf(fy[j], P[j], Q[j]));   // sc = gamma*invstd
     }
   };
@@ -381,6 +395,7 @@ static inline unsigned bn_grid(long work_threads, long cap) {
   long b = (work_threads + BN_THREADS - 1) / BN_THREADS;
   return (unsigned)(b > cap ? cap : (b < 1 ? 1 : b));
 }
+static inline bool bn_act_ok(int act) { return act == 0 || act == 1 || act == 2 || act == 4; }
 static inline bool bn_c_ok(int C) { return C >= 8 && C % 8 == 0 && (C / 8) <= BN_THREADS && ((C / 8) & (C / 8 - 1)) == 0; }
 
 static inline long bn_reduce_blocks(long M, int C, long wave) {
@@ -396,7 +411,7 @@ static inline long bn_reduce_blocks(long M, int C, long wave) {
 // rows of the partial-sum buffer ([rows][2][C] floats) the reduction kernels need: which = 0 forward stats, 1 backward reduce
 extern "C" int32_t etb_bn_partial_rows(int64_t M, int32_t C, int32_t which) {
   if (M <= 0 || !bn_c_ok(C)) return 0;
-  return (int32_t)bn_reduce_blocks((long)M, C, which ? BN_WAVE(bn_act_bwd_reduce_kernel) : BN_WAVE(bn_stats_kernel));
+  return (int32_t)bn_reduce_blocks((long)M, C, which ? BN_WAVE(bn_act_bwd_reduce_kernel<false>) : BN_WAVE(bn_stats_kernel));
 }
 
 // partials: [rows = etb_bn_partial_rows(M,C,0)][2][C] floats, fully overwritten.  y [M][y_cstride] bf16.
@@ -427,8 +442,13 @@ extern "C" int etb_bn_act_apply_res(const void* y_bf16, const float* scale, cons
                                     void* stream) {
   ETB_CHECK_ARG(y_bf16 && scale && shift && out_bf16 && M > 0 && bn_c_ok(C) && y_cstride % 8 == 0 && out_cstride % 8 == 0);
   ETB_CHECK_ARG(!res_bf16 || (res_cstride % 8 == 0 && res_cstride >= C));
-  etb_launch(bn_act_apply_kernel, dim3(bn_grid(M * (C / 8), BN_WAVE(bn_act_apply_kernel))), dim3(BN_THREADS), 0, (cudaStream_t)stream, (const __nv_bfloat16*)y_bf16, scale, shift, (__nv_bfloat16*)out_bf16, (long)M, C, y_cstride, out_cstride, act,
-      (const __nv_bfloat16*)res_bf16, res_cstride);
+  ETB_CHECK_ARG(bn_act_ok(act));
+  if (act == 4)
+    etb_launch(bn_act_apply_kernel<true>, dim3(bn_grid(M * (C / 8), BN_WAVE(bn_act_apply_kernel<true>))), dim3(BN_THREADS), 0, (cudaStream_t)stream, (const __nv_bfloat16*)y_bf16, scale, shift, (__nv_bfloat16*)out_bf16, (long)M, C, y_cstride, out_cstride, act,
+        (const __nv_bfloat16*)res_bf16, res_cstride);
+  else
+    etb_launch(bn_act_apply_kernel<false>, dim3(bn_grid(M * (C / 8), BN_WAVE(bn_act_apply_kernel<false>))), dim3(BN_THREADS), 0, (cudaStream_t)stream, (const __nv_bfloat16*)y_bf16, scale, shift, (__nv_bfloat16*)out_bf16, (long)M, C, y_cstride, out_cstride, act,
+        (const __nv_bfloat16*)res_bf16, res_cstride);
   ETB_CHECK_LAUNCH();
   return ETB_OK;
 }
@@ -442,8 +462,8 @@ extern "C" int etb_bn_act_bwd_reduce(const void* da_bf16, const void* y_bf16, co
                                      const float* invstd, int64_t M, int32_t C, int32_t da_cstride, int32_t y_cstride, int32_t act,
                                      float* partials, int32_t rows, void* stream) {
   ETB_CHECK_ARG(da_bf16 && y_bf16 && scale && shift && mean && invstd && partials && M > 0 && M < (1ll << 31) && bn_c_ok(C));
-  ETB_CHECK_ARG(da_cstride % 8 == 0 && y_cstride % 8 == 0 && rows == etb_bn_partial_rows(M, C, 1));
-  etb_launch(bn_act_bwd_reduce_kernel, dim3((unsigned)rows), dim3(BN_THREADS), 0, (cudaStream_t)stream, (const __nv_bfloat16*)da_bf16, (const __nv_bfloat16*)y_bf16, scale, shift, mean, invstd, (int)M, C, da_cstride, y_cstride, act, partials);
+  ETB_CHECK_ARG(da_cstride % 8 == 0 && y_cstride % 8 == 0 && rows == etb_bn_partial_rows(M, C, 1) && bn_act_ok(act));
+  etb_launch(act == 4 ? bn_act_bwd_reduce_kernel<true> : bn_act_bwd_reduce_kernel<false>, dim3((unsigned)rows), dim3(BN_THREADS), 0, (cudaStream_t)stream, (const __nv_bfloat16*)da_bf16, (const __nv_bfloat16*)y_bf16, scale, shift, mean, invstd, (int)M, C, da_cstride, y_cstride, act, partials);
   ETB_CHECK_LAUNCH();
   return ETB_OK;
 }
@@ -465,9 +485,13 @@ extern "C" int etb_bn_act_bwd_apply(const void* da_bf16, const void* y_bf16, con
                                     const float* invstd, const float* sums, int64_t M, int32_t C, int32_t da_cstride, int32_t y_cstride,
                                     int32_t dy_cstride, int32_t act, void* dy_bf16, void* stream) {
   ETB_CHECK_ARG(da_bf16 && y_bf16 && scale && shift && mean && invstd && sums && dy_bf16 && M > 0 && bn_c_ok(C));
-  ETB_CHECK_ARG(da_cstride % 8 == 0 && y_cstride % 8 == 0 && dy_cstride % 8 == 0);
-  etb_launch(bn_act_bwd_apply_kernel, dim3(bn_grid(M * (C / 8), BN_WAVE(bn_act_bwd_apply_kernel))), dim3(BN_THREADS), 0, (cudaStream_t)stream, (const __nv_bfloat16*)da_bf16, (const __nv_bfloat16*)y_bf16, scale, shift, mean, invstd, sums, (long)M, C, da_cstride, y_cstride, dy_cstride,
-      act, (__nv_bfloat16*)dy_bf16);
+  ETB_CHECK_ARG(da_cstride % 8 == 0 && y_cstride % 8 == 0 && dy_cstride % 8 == 0 && bn_act_ok(act));
+  if (act == 4)
+    etb_launch(bn_act_bwd_apply_kernel<true>, dim3(bn_grid(M * (C / 8), BN_WAVE(bn_act_bwd_apply_kernel<true>))), dim3(BN_THREADS), 0, (cudaStream_t)stream, (const __nv_bfloat16*)da_bf16, (const __nv_bfloat16*)y_bf16, scale, shift, mean, invstd, sums, (long)M, C, da_cstride, y_cstride, dy_cstride,
+        act, (__nv_bfloat16*)dy_bf16);
+  else
+    etb_launch(bn_act_bwd_apply_kernel<false>, dim3(bn_grid(M * (C / 8), BN_WAVE(bn_act_bwd_apply_kernel<false>))), dim3(BN_THREADS), 0, (cudaStream_t)stream, (const __nv_bfloat16*)da_bf16, (const __nv_bfloat16*)y_bf16, scale, shift, mean, invstd, sums, (long)M, C, da_cstride, y_cstride, dy_cstride,
+        act, (__nv_bfloat16*)dy_bf16);
   ETB_CHECK_LAUNCH();
   return ETB_OK;
 }

@@ -61,6 +61,14 @@ static inline int etb_num_sms() {
   return sms;
 }
 
+// `act` codes of the BatchNorm kernels (bn.cu) and of the folded-BN conv epilogue (conv_wgmma.cu): 0 none, 1 SiLU,
+// 2 ReLU, 4 Hardswish.  3 is not used: older documentation of etb_conv_dgrad gave it the meaning "accumulate into dx".
+
+// nn.Hardswish, as torch computes it on the CPU: z * min(max(z + 3, 0), 6) / 6
+__device__ __forceinline__ float hswish_f(float z) { return z * fminf(fmaxf(z + 3.0f, 0.0f), 6.0f) / 6.0f; }
+// its derivative as torch's hardswish_backward takes it: 0 for z <= -3, z/3 + 1/2 strictly between -3 and 3, 1 for z >= 3
+__device__ __forceinline__ float dhswish_f(float z) { return z <= -3.0f ? 0.0f : (z < 3.0f ? z / 3.0f + 0.5f : 1.0f); }
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

@@ -163,7 +163,7 @@ struct ConvKArgs {
   int Ho, Wo, Cout;
   int y_cstride, y_coffset;
   int res_cstride, res_coffset;
-  int act;                // 0 none, 1 SiLU, 2 ReLU
+  int act;                // 0 none, 1 SiLU, 2 ReLU (EPI 1), 4 Hardswish (EPI 3)
   int out_mode;           // 0: bf16 NHWC ; 1: fp32 Detect layout [N, na, Ho, Wo, no] with c = a*no + o
   int det_no, det_hw;     // outputs per anchor, pixels per image (Detect layout)
   const float* scale;     // [Cout] or null (=1)
@@ -195,6 +195,8 @@ __device__ __forceinline__ float conv_act(float x, int act) {
 //   EPI 0: raw bf16 store (+= existing when a.accumulate)       -- dgrad, training forward
 //   EPI 1: v*scale+bias (folded BN) -> SiLU/ReLU -> (+residual) -- teacher forward
 //   EPI 2: +bias, fp32 scatter into the Detect layout           -- head
+//   EPI 3: EPI 1 with Hardswish                                 -- teacher forward of Hardswish layers
+// (Hardswish as a third run-time case of EPI 1 would raise the SiLU instances from 122 / 89 to 132 / 98 registers.)
 template <int BN, int EPI>
 __device__ __forceinline__ void conv_epilogue(const ConvKArgs& a, const float* d, int n0, const bool* row_ok, const size_t* pix, int lane) {
   const size_t hw = (size_t)a.det_hw;
@@ -205,7 +207,7 @@ __device__ __forceinline__ void conv_epilogue(const ConvKArgs& a, const float* d
     if (gc >= a.Cout) continue;
     const bool pair = gc + 1 < a.Cout;
     float sc0 = 1.f, sc1 = 1.f, bi0 = 0.f, bi1 = 0.f;
-    if (EPI == 1 && a.scale) { sc0 = __ldg(a.scale + gc); sc1 = pair ? __ldg(a.scale + gc + 1) : 1.f; }
+    if ((EPI == 1 || EPI == 3) && a.scale) { sc0 = __ldg(a.scale + gc); sc1 = pair ? __ldg(a.scale + gc + 1) : 1.f; }
     if (EPI != 0 && a.bias) { bi0 = __ldg(a.bias + gc); bi1 = pair ? __ldg(a.bias + gc + 1) : 0.f; }
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
@@ -223,9 +225,9 @@ __device__ __forceinline__ void conv_epilogue(const ConvKArgs& a, const float* d
         continue;
       }
       __nv_bfloat16* yp = a.y + pix[i] * a.y_cstride + a.y_coffset + gc;
-      if (EPI == 1) {
-        v0 = conv_act(fmaf(v0, sc0, bi0), a.act);
-        v1 = conv_act(fmaf(v1, sc1, bi1), a.act);
+      if (EPI == 1 || EPI == 3) {
+        v0 = EPI == 3 ? hswish_f(fmaf(v0, sc0, bi0)) : conv_act(fmaf(v0, sc0, bi0), a.act);
+        v1 = EPI == 3 ? hswish_f(fmaf(v1, sc1, bi1)) : conv_act(fmaf(v1, sc1, bi1), a.act);
         if (a.residual) {     // Cout % 8 == 0 whenever a shortcut is fused: the pair is whole
           const float2 rf = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(a.residual + pix[i] * a.res_cstride + a.res_coffset + gc));
           v0 += rf.x;
@@ -397,6 +399,7 @@ static int launch_conv_e(const CUtensorMap& mA, const CUtensorMap& mB, const Con
 template <int BN>
 static int launch_conv(const CUtensorMap& mA, const CUtensorMap& mB, const ConvKArgs& ka, dim3 grid, cudaStream_t st) {
   if (ka.out_mode == 1) return launch_conv_e<BN, 2>(mA, mB, ka, grid, st);
+  if (ka.act == 4) return launch_conv_e<BN, 3>(mA, mB, ka, grid, st);
   if (ka.scale || ka.bias || ka.act || ka.residual) return launch_conv_e<BN, 1>(mA, mB, ka, grid, st);
   return launch_conv_e<BN, 0>(mA, mB, ka, grid, st);
 }
@@ -488,6 +491,7 @@ extern "C" int etb_conv_fwd(const void* x_bf16, const void* w_bf16, const float*
   (void)workspace; (void)workspace_bytes;
   ETB_CHECK_ARG(x_bf16 && w_bf16 && cp && (y_bf16 || y_f32));
   ETB_CHECK_ARG(cp->N > 0 && cp->H > 0 && cp->W > 0 && cp->Cin > 0 && cp->Cout > 0);
+  ETB_CHECK_ARG(cp->act == 0 || cp->act == 1 || cp->act == 2 || cp->act == 4);
   ETB_CHECK_ARG(cp->kh >= 1 && cp->kw >= 1 && cp->kh * cp->kw <= 12 && (cp->stride == 1 || cp->stride == 2) && cp->pad >= 0);
   const int Ho = (cp->H + 2 * cp->pad - cp->kh) / cp->stride + 1;
   const int Wo = (cp->W + 2 * cp->pad - cp->kw) / cp->stride + 1;
@@ -584,7 +588,8 @@ extern "C" int etb_pack_weight_dgrad(const float* w_oihw, void* out_bf16, int32_
 
 // dy [N,Ho,Wo,*] bf16 (channels [dy_coffset.. +Cout) of stride dy_cstride) -> dx [N,H,W,*] bf16 at channel offset.
 // cp describes the FORWARD conv (N,H,W,Cin,Cout,k,stride,pad); x_cstride/ y_* name the dy / dx buffers:
-//   cp->x_cstride = channel stride of dy, cp->y_cstride/y_coffset = geometry of dx.  cp->act==3 -> dx += (accumulate).
+//   cp->x_cstride = channel stride of dy, cp->y_cstride/y_coffset = geometry of dx; cp->act is not read.
+//   accumulate != 0 -> dx += result.
 extern "C" int etb_conv_dgrad(const void* dy_bf16, const void* wd_bf16, void* dx_bf16, const EtbConvParams* cp, int32_t accumulate,
                               void* stream) {
   ETB_CHECK_ARG(dy_bf16 && wd_bf16 && dx_bf16 && cp);

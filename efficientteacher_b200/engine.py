@@ -4,15 +4,15 @@
 Data layout: every activation is NHWC bf16 in HBM.  torch.cat never happens: producers write straight into the
 channel slice of the consumer's concat buffer (C3's [m(cv1(x)), cv2(x)], SPPF's [x,y1,y2,y3], the PANet concats),
 and the 2x nearest upsample writes into its slice too.  BatchNorm (eval) is folded into a per-channel scale/bias
-applied, with SiLU and the Bottleneck shortcut, in the convolution epilogue.  The Detect 1x1 convs write fp32
+applied, with the activation (SiLU, ReLU or Hardswish) and the Bottleneck shortcut, in the convolution epilogue.  The Detect 1x1 convs write fp32
 logits directly in the [B,na,ny,nx,no] layout, and the eval decode writes the concatenated [B,P,no] prediction.
 """
 import torch
-import torch.nn as nn
 
 from . import _lib
 from . import convops as co
 from .head import decode_levels
+from .model import native_act
 
 
 class _ConvParams:
@@ -25,8 +25,7 @@ class _ConvParams:
         self.bn = getattr(mod, "bn", None)
         self.Cout, self.Cin = conv.weight.shape[0], conv.weight.shape[1]
         self.k, self.s, self.p = conv.kernel_size[0], conv.stride[0], conv.padding[0]
-        act = getattr(mod, "act", None)
-        self.act = "silu" if isinstance(act, nn.SiLU) else ("relu" if isinstance(act, nn.ReLU) else None)
+        self.act = native_act(getattr(mod, "act", None))
         self.w = self.scale = self.bias = None
 
     def register(self, packer):

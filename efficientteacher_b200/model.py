@@ -7,7 +7,7 @@ Execution:
   * eval / no-grad forward (the teacher-EMA pass of trainer/ssod_trainer.py:595-599) runs on the native engine
     (engine.TrunkEngine: wgmma implicit-GEMM convs, NHWC bf16, BN folded, concat-by-offset, fused Detect).
   * training forward/backward: torch autograd only sequences the graph; every node is a native Function
-    (autograd_conv.ConvBnActFn = wgmma conv + fused BatchNorm(train)+SiLU(+shortcut), JoinFn / SppfPoolFn /
+    (autograd_conv.ConvBnActFn = wgmma conv + fused BatchNorm(train)+activation(+shortcut), JoinFn / SppfPoolFn /
     UpsampleIntoFn = concat-by-offset glue of csrc/glue.cu, DetectConvFn), tensors stay NHWC bf16 and are exposed to
     torch as channels_last views.
 There is no CPU path: forward raises without a CUDA device + libetb200.so.
@@ -29,16 +29,51 @@ def autopad(k, p=None):
     return k // 2 if p is None else p
 
 
+# activation module -> convops.ACT key of the native kernels (the modules get_activation of common.py:28-47 builds)
+NATIVE_ACTS = ((nn.SiLU, "silu"), (nn.ReLU, "relu"), (nn.Hardswish, "hard_swish"))
+
+
+def native_act(m):
+    """convops.ACT key of activation module m; None (no activation) for nn.Identity or any other module"""
+    return next((name for t, name in NATIVE_ACTS if isinstance(m, t)), None)
+
+
+def trunk_acts(activation):
+    """(CONV_ACT, C_ACT) of a cfg.Model.{Backbone,Neck}.activation string (yolov5_backbone.py:47-55, yolov5_neck.py:48-56):
+    'SiLU' and 'ReLU' run everywhere; any other string selects Hardswish for the plain convs and SPPF and the mixed
+    'relu_hswish' C3."""
+    if activation == 'SiLU':
+        return 'silu', 'silu'
+    if activation == 'ReLU':
+        return 'relu', 'relu'
+    return 'hard_swish', 'relu_hswish'
+
+
+def _split_act(act):
+    """C3 / SPPF (common.py:566-592, 682-700): 'relu_hswish' = ReLU in the inner convs, Hardswish in the last one"""
+    return ('relu', 'hard_swish') if act == 'relu_hswish' else (act, act)
+
+
 class Conv(nn.Module):
-    """conv2d(bias=False) + BatchNorm2d(eps 1e-3, momentum 0.03) + SiLU   (common.py:471-484, torch_utils.py:168-169)"""
+    """conv2d(bias=False) + BatchNorm2d(eps 1e-3, momentum 0.03) + SiLU / ReLU / Hardswish   (common.py:471-484,
+    torch_utils.py:168-169)"""
 
     def __init__(self, c1, c2, k=1, s=1, p=None, g=1, act=True):
         super().__init__()
         assert g == 1
         self.conv = nn.Conv2d(c1, c2, k, s, autopad(k, p), groups=g, bias=False)
         self.bn = nn.BatchNorm2d(c2, eps=1e-3, momentum=0.03)
-        self.act = nn.SiLU() if act is True or act == "silu" else (nn.ReLU(inplace=True) if act == "relu" else nn.Identity())
-        self.act_name = "relu" if act == "relu" else None
+        if act is True or act == "silu":
+            self.act = nn.SiLU()
+        elif act == "relu":
+            self.act = nn.ReLU(inplace=True)
+        elif act == "hard_swish":
+            self.act = nn.Hardswish(inplace=True)
+        elif isinstance(act, str):
+            raise NotImplementedError("activation %r is not on the hot path" % act)
+        else:
+            self.act = nn.Identity()
+        self.act_name = act if act in ("relu", "hard_swish") else None
 
     def __deepcopy__(self, memo):   # `_packed` aliases the owning model's packer buffers: copies start without it
         from copy import deepcopy
@@ -55,7 +90,7 @@ class Conv(nn.Module):
         return s
 
     NATIVE = True        # training convs on the wgmma fwd/dgrad/wgrad kernels (False: torch/cuDNN scaffold)
-    FUSED_BN = True      # BatchNorm(train)+SiLU forward/backward on the fused kernels of csrc/bn.cu (False: torch ops)
+    FUSED_BN = True      # BatchNorm(train)+activation forward/backward on the fused kernels of csrc/bn.cu (False: torch ops)
     FUSED_GLUE = True    # concat-by-offset / fused shortcut add / native pool+upsample (csrc/glue.cu) instead of torch ops
     FUSED_FANIN = True   # gradient fan-in (C3 input, shortcut, backbone feature) accumulated in the dgrad epilogue
     is_stem = False
@@ -64,10 +99,10 @@ class Conv(nn.Module):
         """True when this Conv runs as ONE ConvBnActFn (and can therefore write into a CatBuf slice / add a shortcut)."""
         c = self.conv.out_channels
         # csrc/bn.cu (bn_c_ok): one thread owns 8 channels and C/8 must be a power of two <= 256; other widths (YOLOv5m:
-        # 48/96/192/...) run the native conv + torch BatchNorm/SiLU scaffold below instead of raising
+        # 48/96/192/...) run the native conv + torch BatchNorm/activation scaffold below instead of raising
         bn_ok = c % 8 == 0 and (c // 8) & (c // 8 - 1) == 0 and c // 8 <= 256
         return (Conv.NATIVE and Conv.FUSED_BN and bn_ok and x.is_cuda and self.training
-                and isinstance(self.act, (nn.SiLU, nn.ReLU)))
+                and native_act(self.act) is not None)
 
     def glue(self, x):
         return Conv.FUSED_GLUE and self.fused(x) and self.conv.out_channels % 8 == 0
@@ -83,8 +118,8 @@ class Conv(nn.Module):
             wp, wd = (None, None) if pc is None else (pc.fwd, pc.dgrad)
             if self.fused(x):
                 bn = self.bn
-                act = "silu" if isinstance(self.act, nn.SiLU) else "relu"
-                return ConvBnActFn.apply(x, w, bn.weight, bn.bias, bn.running_mean, bn.running_var, s, p, bn.eps, bn.momentum, act,
+                return ConvBnActFn.apply(x, w, bn.weight, bn.bias, bn.running_mean, bn.running_var, s, p, bn.eps, bn.momentum,
+                                         native_act(self.act),
                                          self.is_stem, wp, wd, res, dest, coff)
             assert dest is None
             y = self.act(self.bn(ConvFn.apply(x, w, s, p, self.is_stem, wp, wd)))
@@ -124,9 +159,10 @@ class C3(nn.Module):
     def __init__(self, c1, c2, n=1, shortcut=True, g=1, e=0.5, act=True):
         super().__init__()
         c_ = int(c2 * e)
+        act, last_act = _split_act(act)
         self.cv1 = Conv(c1, c_, 1, 1, act=act)
         self.cv2 = Conv(c1, c_, 1, 1, act=act)
-        self.cv3 = Conv(2 * c_, c2, 1, act=act)
+        self.cv3 = Conv(2 * c_, c2, 1, act=last_act)
         self.m = nn.Sequential(*[Bottleneck(c_, c_, shortcut, g, e=1.0, act=act) for _ in range(n)])
 
     def forward(self, x):
@@ -148,8 +184,9 @@ class SPPF(nn.Module):
     def __init__(self, c1, c2, k=5, act=True):
         super().__init__()
         c_ = c1 // 2
+        act, last_act = _split_act(act)
         self.cv1 = Conv(c1, c_, 1, 1, act=act)
-        self.cv2 = Conv(c_ * 4, c2, 1, 1, act=act)
+        self.cv2 = Conv(c_ * 4, c2, 1, 1, act=last_act)
         self.m = nn.MaxPool2d(kernel_size=k, stride=1, padding=k // 2)
 
     def forward(self, x):
@@ -180,20 +217,18 @@ class YoloV5BackBone(nn.Module):
         self.gd, self.gw = cfg.Model.depth_multiple, cfg.Model.width_multiple
         w = lambda n: make_divisible(n * self.gw, 8)  # noqa: E731
         d = lambda n: max(round(n * self.gd), 1) if n > 1 else n  # noqa: E731
-        act = 'silu' if cfg.Model.Backbone.activation == 'SiLU' else None
-        if act is None:
-            raise NotImplementedError("only SiLU YOLOv5 trunks are on the hot path")
+        act, c_act = trunk_acts(cfg.Model.Backbone.activation)
         c1, c2, c3, c4, c5 = w(64), w(128), w(256), w(512), w(1024)
         self.stage1 = Conv(3, c1, 6, 2, 2, 1, act)
         self.stage1.is_stem = True
         self.stage2_1 = Conv(c1, c2, 3, 2, None, 1, act)
-        self.stage2_2 = C3(c2, c2, d(3), True, 1, 0.5, act)
+        self.stage2_2 = C3(c2, c2, d(3), True, 1, 0.5, c_act)
         self.stage3_1 = Conv(c2, c3, 3, 2, None, 1, act)
-        self.stage3_2 = C3(c3, c3, d(6), True, 1, 0.5, act)
+        self.stage3_2 = C3(c3, c3, d(6), True, 1, 0.5, c_act)
         self.stage4_1 = Conv(c3, c4, 3, 2, None, 1, act)
-        self.stage4_2 = C3(c4, c4, d(9), True, 1, 0.5, act)
+        self.stage4_2 = C3(c4, c4, d(9), True, 1, 0.5, c_act)
         self.stage5_1 = Conv(c4, c5, 3, 2, None, 1, act)
-        self.stage5_2 = C3(c5, c5, d(3), True, 1, 0.5, act)
+        self.stage5_2 = C3(c5, c5, d(3), True, 1, 0.5, c_act)
         self.sppf = SPPF(c5, c5, 5, act)
         self.out_shape = {'C3_size': c3, 'C4_size': c4, 'C5_size': c5}
 
@@ -218,19 +253,17 @@ class YoloV5Neck(nn.Module):
         op3, op4, op5 = [w(c) for c in cfg.Model.Neck.out_channels]
         self.input_p3, self.input_p4, self.input_p5 = ip3, ip4, ip5
         self.output_p3, self.output_p4, self.output_p5 = op3, op4, op5
-        act = 'silu' if cfg.Model.Neck.activation == 'SiLU' else None
-        if act is None:
-            raise NotImplementedError("only SiLU YOLOv5 trunks are on the hot path")
+        act, c_act = trunk_acts(cfg.Model.Neck.activation)
         self.conv1 = Conv(ip5, int(ip5 / 2), 1, 1, None, 1, act)
         self.upsample1 = nn.Upsample(scale_factor=2, mode="nearest")
-        self.C1 = C3(int(ip5 / 2) + ip4, ip4, d(3), False, 1, 0.5, act)
+        self.C1 = C3(int(ip5 / 2) + ip4, ip4, d(3), False, 1, 0.5, c_act)
         self.conv2 = Conv(ip4, ip3, 1, 1, None, 1, act)
         self.upsample2 = nn.Upsample(scale_factor=2, mode="nearest")
-        self.C2 = C3(ip3 + ip3, op3, d(3), False, 1, 0.5, act)
+        self.C2 = C3(ip3 + ip3, op3, d(3), False, 1, 0.5, c_act)
         self.conv3 = Conv(op3, op3, 3, 2, None, 1, act)
-        self.C3 = C3(op3 + ip3, op4, d(3), False, 1, 0.5, act)
+        self.C3 = C3(op3 + ip3, op4, d(3), False, 1, 0.5, c_act)
         self.conv4 = Conv(op4, op4, 3, 2, None, 1, act)
-        self.C4 = C3(op4 + int(ip5 / 2), op5, d(3), False, 1, 0.5, act)
+        self.C4 = C3(op4 + int(ip5 / 2), op5, d(3), False, 1, 0.5, c_act)
         self.concat = Concat()
 
     def _up_cat(self, x, lateral):

@@ -207,7 +207,8 @@ int etb_loss_backward(const float* const* p, float* const* grad_p, const EtbLoss
  * place), w [Cout, kh*kw*Cin] bf16 (K-major), y [N,Ho,Wo,*] bf16 written at channel offset into a buffer
  * with y_cstride channels (so concat is free).
  *   epilogue: v = acc*scale[c] + bias[c]  (folded eval-mode BN, or conv bias with scale=NULL)
- *             act 0: none, 1: SiLU, 2: ReLU ;  optional residual add (Bottleneck shortcut) after act.
+ *             act 0: none, 1: SiLU, 2: ReLU, 4: Hardswish (3 is not a code) ;  optional residual add (Bottleneck
+ *             shortcut) after act.
  *   y_f32 != NULL: write fp32 in the Detect train layout [N,na,Ho,Wo,det_no] instead (channel c = a*det_no+o).
  * ------------------------------------------------------------------------------------------- */
 typedef struct EtbConvParams {
@@ -215,7 +216,7 @@ typedef struct EtbConvParams {
   int32_t kh, kw, stride, pad;
   int32_t x_cstride, y_cstride, y_coffset; /* channel strides of the NHWC buffers, output channel offset */
   int32_t res_cstride, res_coffset;        /* residual buffer geometry (if residual != NULL) */
-  int32_t act;                             /* 0 none, 1 SiLU, 2 ReLU */
+  int32_t act;                             /* 0 none, 1 SiLU, 2 ReLU, 4 Hardswish; etb_conv_dgrad/wgrad ignore it */
   int32_t det_no;                          /* y_f32 path: outputs per anchor (85); Cout = na*det_no */
 } EtbConvParams;
 
@@ -244,9 +245,11 @@ size_t etb_conv_wgrad_workspace_bytes(const EtbConvParams* cp);
 int etb_conv_wgrad(const void* x_bf16, const void* dy_bf16, float* dw_f32, const EtbConvParams* cp, int32_t flags,
                    void* workspace, size_t workspace_bytes, void* stream);
 
-/* training-mode BatchNorm2d (eps, momentum, batch statistics, running-stat update with the unbiased variance) + SiLU/ReLU
+/* training-mode BatchNorm2d (eps, momentum, batch statistics, running-stat update with the unbiased variance) + activation
  * around the convolutions (models/backbone/common.py:480-481; utils/torch_utils.py:162-171), forward and backward.
- * y / da / dy / out are NHWC bf16 [M][cstride] with M = N*H*W; per-channel vectors are fp32.  act: 0 none, 1 SiLU, 2 ReLU.
+ * y / da / dy / out are NHWC bf16 [M][cstride] with M = N*H*W; per-channel vectors are fp32.
+ * act: 0 none, 1 SiLU, 2 ReLU (derivative 0 at 0), 4 Hardswish z*min(max(z+3,0),6)/6 (derivative 0 for z <= -3, z/3+1/2
+ * for -3 < z < 3, 1 for z >= 3: torch's hardswish_backward); any other value is ETB_ERR_INVALID.
  *   forward : etb_bn_stats (per-block partial rows [rows][2][C] = sum y, sum y^2; rows = etb_bn_partial_rows(M,C,0))
  *             -> etb_bn_finalize (fixed-order sum of the rows -> scale, shift, mean, invstd, running stats)
  *             -> etb_bn_act_apply (a = act(y*scale+shift))
