@@ -36,10 +36,16 @@ def _ssod():
               extra_teachers=[], multi_step_lr=False)
 
 
+# (depth_multiple, width_multiple) of the reference's five YOLOv5 sizes (configs/sup/public/yolov5{n,s,m,l,x}_coco.yaml),
+# plus shallow variants (depth 0.33: one or two Bottlenecks per C3) that keep a size's widths for quick tests
+SIZES = {'n': (0.33, 0.25), 's': (0.33, 0.50), 'm': (0.67, 0.75), 'l': (1.0, 1.0), 'x': (1.33, 1.25),
+         'l_shallow': (0.33, 1.0), 'm_shallow': (0.33, 0.75), 'x_shallow': (0.33, 1.25)}
+
+
 def yolov5_ssod_cfg(size='l', batch_size=32, img_size=640, backbone_act='SiLU', neck_act='SiLU'):
     """backbone_act / neck_act: cfg.Model.{Backbone,Neck}.activation -- 'SiLU', 'ReLU', or anything else for the Hardswish
     trunk (the reference's defaults, configs/defaults.py, are 'LeakyReLU' and 'ReLU': a Hardswish backbone, a ReLU neck)"""
-    depth, width = {'l': (1.0, 1.0), 's': (0.33, 0.50), 'm': (0.67, 0.75), 'l_shallow': (0.33, 1.0)}[size]
+    depth, width = SIZES[size]
     return NS(epochs=300, adam=False, linear_lr=True, single_cls=False, sync_bn=False,
               hyp=_hyp(), Model=_model(depth, width, backbone_act, neck_act), Loss=_loss(), SSOD=_ssod(),
               Dataset=NS(nc=80, np=0, names=list(COCO_NAMES), img_size=img_size, batch_size=batch_size))

@@ -48,10 +48,11 @@ __device__ __forceinline__ void store8(__nv_bfloat16* p, const float* f) {
   *reinterpret_cast<uint4*>(p) = v;
 }
 
-// Per-channel reduction of up to two quantities.  Thread t owns channel group g = t % G (G = C/8 divides 256) and
-// pixel lane t / G; rows advance by (256/G)*gridDim.x so g never changes.  Block partials are combined through shared
-// memory and written to out[blockIdx.x][NQ][C]: no atomics, no memset, and the second stage (reduce_partials) sums the
-// rows in a fixed order, so the statistics are bit-reproducible run to run.
+// Per-channel reduction of up to two quantities.  Thread t owns channel group g = t % G (G = C/8 <= 256) and pixel lane
+// t / G; rows advance by PL*gridDim.x with PL = floor(256/G), so g never changes.  When G does not divide 256 (YOLOv5m/x
+// widths) the last 256 - PL*G threads own no lane and stay idle.  Block partials are combined through shared memory and
+// written to out[blockIdx.x][NQ][C]: no atomics, no memset, and the second stage (reduce_partials) sums the rows in a
+// fixed order, so the statistics are bit-reproducible run to run.
 template <int NQ, int UNROLL, typename D, typename L, typename F>
 __device__ __forceinline__ void channel_reduce(int M, int C, L&& load_row, F&& per_row, float* __restrict__ out /*[NQ][C]*/) {
   __shared__ float sh[NQ][BN_THREADS][8 + 1];
@@ -63,7 +64,7 @@ __device__ __forceinline__ void channel_reduce(int M, int C, L&& load_row, F&& p
 #pragma unroll
     for (int j = 0; j < 8; ++j) acc[q][j] = 0.f;
   const int step = (int)gridDim.x * PL;
-  int r = (int)blockIdx.x * PL + pl;
+  int r = pl < PL ? (int)blockIdx.x * PL + pl : M;
   for (; r + (UNROLL - 1) * step < M; r += UNROLL * step) {      // UNROLL independent rows in flight per thread
     D d[UNROLL];
 #pragma unroll
@@ -196,20 +197,42 @@ __device__ __forceinline__ float bn_dact(float z, int act) {   // ReLU'(0) = 0, 
   return HSWISH ? dhswish_f(z) : (act == 1 ? dsilu_f(z) : (act == 2 ? (z > 0.f ? 1.f : 0.f) : 1.f));
 }
 
+// Index space of the apply kernels, in which every thread keeps one channel group g for its whole life.
+//   POW2 (G = C/8 a power of two): e counts 16 B vectors, row = e >> lg; the grid stride (gridDim.x*256 vectors) is a
+//     multiple of G, so g = e & (G-1) never changes.
+//   otherwise (YOLOv5m/x widths): thread t owns g = t % G and row lane t / G < PL = floor(256/G), as in channel_reduce;
+//     e counts rows (lg = 0) and advances by PL*gridDim.x.  The 256 - PL*G tail threads of a block return at once.
+// Either way the loop body needs no division.  Returns false for an idle thread.
+template <bool POW2>
+__device__ __forceinline__ bool bn_apply_index(long M, int C, int* g, int* lg, long* e, long* stride, long* total) {
+  const int G = C >> 3;
+  if (POW2) {
+    *lg = 31 - __clz(G);
+    *total = M * G;
+    *stride = (long)gridDim.x * blockDim.x;
+    *e = (long)blockIdx.x * blockDim.x + threadIdx.x;
+    *g = (int)(*e & (G - 1));
+    return true;
+  }
+  const int PL = BN_THREADS / G, pl = threadIdx.x / G;
+  *lg = 0;
+  *total = M;
+  *stride = (long)gridDim.x * PL;
+  *e = (long)blockIdx.x * PL + pl;
+  *g = threadIdx.x - pl * G;
+  return pl < PL;
+}
+
 // ---- forward apply: a = act(y*scale + shift) ----
-// The grid stride (gridDim.x*256 vectors) is a multiple of G = C/8 (a power of two <= 256), so a thread's channel group
-// never changes: its scale/shift live in registers for the whole kernel and the loop body is 2 independent 16 B loads,
-// 8 FMAs + SiLU, 2 stores.
-template <bool HSWISH>
+// A thread's channel group never changes (bn_apply_index): its scale/shift live in registers for the whole kernel and the
+// loop body is 2 independent 16 B loads, 8 FMAs + SiLU, 2 stores.
+template <bool HSWISH, bool POW2>
 __global__ void __launch_bounds__(BN_THREADS) bn_act_apply_kernel(const __nv_bfloat16* __restrict__ y, const float* __restrict__ scale,
                                                                   const float* __restrict__ shift, __nv_bfloat16* __restrict__ out, long M, int C,
                                                                   int ycs, int ocs, int act, const __nv_bfloat16* __restrict__ res, int rcs) {
-  const int G = C >> 3;
-  const int lg = 31 - __clz(G);            // G is a power of two (checked on the host): no 64-bit divisions
-  const long total = M * G;
-  const long stride = (long)gridDim.x * blockDim.x;
-  long e = (long)blockIdx.x * blockDim.x + threadIdx.x;
-  const int g = (int)(e & (G - 1));
+  int g, lg;
+  long e, stride, total;
+  if (!bn_apply_index<POW2>(M, C, &g, &lg, &e, &stride, &total)) return;
   float sc[8], sh[8];
   ldf8(scale + g * 8, sc); ldf8(shift + g * 8, sh);
   y += g * 8;
@@ -310,19 +333,16 @@ __global__ void __launch_bounds__(BNR_CH * BNR_GR) bn_bwd_finalize_kernel(const 
 // ---- backward apply: dy = gamma*invstd * (dz - sum_dz/M - xhat*sum_dz_xhat/M) ----
 // Same fixed-channel-group structure as the forward apply: the six per-channel vectors are folded into five register
 // arrays once per thread.
-template <bool HSWISH>
+template <bool HSWISH, bool POW2>
 __global__ void __launch_bounds__(BN_THREADS, 2) bn_act_bwd_apply_kernel(const __nv_bfloat16* __restrict__ da, const __nv_bfloat16* __restrict__ y,
                                                                       const float* __restrict__ scale, const float* __restrict__ shift,
                                                                       const float* __restrict__ mean, const float* __restrict__ invstd,
                                                                       const float* __restrict__ sums, long M, int C, int dacs, int ycs, int ocs,
                                                                       int act, __nv_bfloat16* __restrict__ dy) {
-  const int G = C >> 3;
-  const int lg = 31 - __clz(G);
-  const long total = M * G;
   const float invM = 1.0f / (float)M;
-  const long stride = (long)gridDim.x * blockDim.x;
-  long e = (long)blockIdx.x * blockDim.x + threadIdx.x;
-  const int g = (int)(e & (G - 1));
+  int g, lg;
+  long e, stride, total;
+  if (!bn_apply_index<POW2>(M, C, &g, &lg, &e, &stride, &total)) return;
   // dy = sc*(dz - k0 - xhat*k1), xhat = y*invstd - mean*invstd  ==>  dy = sc*dz + y*P + Q with
   // P = -sc*invstd*k1, Q = -sc*(k0 - mean*invstd*k1): four register arrays per thread instead of six
   float sc[8], sh[8], P[8], Q[8];
@@ -396,7 +416,27 @@ static inline unsigned bn_grid(long work_threads, long cap) {
   return (unsigned)(b > cap ? cap : (b < 1 ? 1 : b));
 }
 static inline bool bn_act_ok(int act) { return act == 0 || act == 1 || act == 2 || act == 4; }
-static inline bool bn_c_ok(int C) { return C >= 8 && C % 8 == 0 && (C / 8) <= BN_THREADS && ((C / 8) & (C / 8 - 1)) == 0; }
+static inline bool bn_c_ok(int C) { return C >= 8 && C % 8 == 0 && (C / 8) <= BN_THREADS; }
+static inline bool bn_pow2(int C) { return ((C / 8) & (C / 8 - 1)) == 0; }
+// vectors (POW2) or rows (otherwise) of work threads of an apply kernel: both give ceil(M / PL) blocks
+static inline long bn_apply_threads(long M, int C) {
+  const int PL = BN_THREADS / (C / 8);
+  return bn_pow2(C) ? M * (C / 8) : (M + PL - 1) / PL * BN_THREADS;
+}
+// the four instances of an apply kernel: the Hardswish one (act 4) or the run-time SiLU / ReLU / none one, each with the
+// power-of-two or the general channel mapping
+#define BN_APPLY_LAUNCH(kernel, M, C, act, stream, ...)                                                                   \
+  do {                                                                                                                    \
+    const long wt_ = bn_apply_threads((M), (C));                                                                          \
+    if ((act) == 4 && bn_pow2(C))                                                                                         \
+      etb_launch(kernel<true, true>, dim3(bn_grid(wt_, BN_WAVE((kernel<true, true>)))), dim3(BN_THREADS), 0, (stream), __VA_ARGS__);     \
+    else if ((act) == 4)                                                                                                  \
+      etb_launch(kernel<true, false>, dim3(bn_grid(wt_, BN_WAVE((kernel<true, false>)))), dim3(BN_THREADS), 0, (stream), __VA_ARGS__);   \
+    else if (bn_pow2(C))                                                                                                  \
+      etb_launch(kernel<false, true>, dim3(bn_grid(wt_, BN_WAVE((kernel<false, true>)))), dim3(BN_THREADS), 0, (stream), __VA_ARGS__);   \
+    else                                                                                                                  \
+      etb_launch(kernel<false, false>, dim3(bn_grid(wt_, BN_WAVE((kernel<false, false>)))), dim3(BN_THREADS), 0, (stream), __VA_ARGS__); \
+  } while (0)
 
 static inline long bn_reduce_blocks(long M, int C, long wave) {
   const int PL = BN_THREADS / (C / 8);
@@ -443,12 +483,8 @@ extern "C" int etb_bn_act_apply_res(const void* y_bf16, const float* scale, cons
   ETB_CHECK_ARG(y_bf16 && scale && shift && out_bf16 && M > 0 && bn_c_ok(C) && y_cstride % 8 == 0 && out_cstride % 8 == 0);
   ETB_CHECK_ARG(!res_bf16 || (res_cstride % 8 == 0 && res_cstride >= C));
   ETB_CHECK_ARG(bn_act_ok(act));
-  if (act == 4)
-    etb_launch(bn_act_apply_kernel<true>, dim3(bn_grid(M * (C / 8), BN_WAVE(bn_act_apply_kernel<true>))), dim3(BN_THREADS), 0, (cudaStream_t)stream, (const __nv_bfloat16*)y_bf16, scale, shift, (__nv_bfloat16*)out_bf16, (long)M, C, y_cstride, out_cstride, act,
-        (const __nv_bfloat16*)res_bf16, res_cstride);
-  else
-    etb_launch(bn_act_apply_kernel<false>, dim3(bn_grid(M * (C / 8), BN_WAVE(bn_act_apply_kernel<false>))), dim3(BN_THREADS), 0, (cudaStream_t)stream, (const __nv_bfloat16*)y_bf16, scale, shift, (__nv_bfloat16*)out_bf16, (long)M, C, y_cstride, out_cstride, act,
-        (const __nv_bfloat16*)res_bf16, res_cstride);
+  BN_APPLY_LAUNCH(bn_act_apply_kernel, M, C, act, (cudaStream_t)stream, (const __nv_bfloat16*)y_bf16, scale, shift, (__nv_bfloat16*)out_bf16,
+                  (long)M, C, y_cstride, out_cstride, act, (const __nv_bfloat16*)res_bf16, res_cstride);
   ETB_CHECK_LAUNCH();
   return ETB_OK;
 }
@@ -486,12 +522,8 @@ extern "C" int etb_bn_act_bwd_apply(const void* da_bf16, const void* y_bf16, con
                                     int32_t dy_cstride, int32_t act, void* dy_bf16, void* stream) {
   ETB_CHECK_ARG(da_bf16 && y_bf16 && scale && shift && mean && invstd && sums && dy_bf16 && M > 0 && bn_c_ok(C));
   ETB_CHECK_ARG(da_cstride % 8 == 0 && y_cstride % 8 == 0 && dy_cstride % 8 == 0 && bn_act_ok(act));
-  if (act == 4)
-    etb_launch(bn_act_bwd_apply_kernel<true>, dim3(bn_grid(M * (C / 8), BN_WAVE(bn_act_bwd_apply_kernel<true>))), dim3(BN_THREADS), 0, (cudaStream_t)stream, (const __nv_bfloat16*)da_bf16, (const __nv_bfloat16*)y_bf16, scale, shift, mean, invstd, sums, (long)M, C, da_cstride, y_cstride, dy_cstride,
-        act, (__nv_bfloat16*)dy_bf16);
-  else
-    etb_launch(bn_act_bwd_apply_kernel<false>, dim3(bn_grid(M * (C / 8), BN_WAVE(bn_act_bwd_apply_kernel<false>))), dim3(BN_THREADS), 0, (cudaStream_t)stream, (const __nv_bfloat16*)da_bf16, (const __nv_bfloat16*)y_bf16, scale, shift, mean, invstd, sums, (long)M, C, da_cstride, y_cstride, dy_cstride,
-        act, (__nv_bfloat16*)dy_bf16);
+  BN_APPLY_LAUNCH(bn_act_bwd_apply_kernel, M, C, act, (cudaStream_t)stream, (const __nv_bfloat16*)da_bf16, (const __nv_bfloat16*)y_bf16, scale,
+                  shift, mean, invstd, sums, (long)M, C, da_cstride, y_cstride, dy_cstride, act, (__nv_bfloat16*)dy_bf16);
   ETB_CHECK_LAUNCH();
   return ETB_OK;
 }

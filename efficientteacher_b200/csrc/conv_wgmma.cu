@@ -886,13 +886,14 @@ __global__ void __launch_bounds__(32 * SG) wgrad_reduce_kernel(const float* __re
 // and 64 consecutive ci: unit (tap, lane) sums its float4 over the slices (coalesced along ci), the [64][kk] patch is
 // transposed through shared memory and written (or accumulated) as ONE contiguous run of 64*kk floats -- the naive
 // scatter cost 8x sector amplification on both the read-modify-write and the store (60 us per 3x3 layer).
+// When Cin % 64 != 0 (YOLOv5m: 96, YOLOv5x: 80, 160, ...) the last chunk of a co holds the remaining Cin % 64 channels.
 __global__ void __launch_bounds__(256) wgrad_reduce_taps_kernel(const float* __restrict__ ws, long slice, int splitk, float* __restrict__ out, int Cin,
                                                                 int kk, int flags) {
   __shared__ float sm[64 * 12];
-  const int CW = Cin < 64 ? Cin : 64;            // channels per block (Cin is a multiple of 64, or smaller than 64 and of 8)
+  const int chunks = (Cin + 63) >> 6;
+  const int co = blockIdx.x / chunks, ci0 = (blockIdx.x - co * chunks) * 64;
+  const int CW = min(Cin - ci0, 64);             // channels of this block, a multiple of 8
   const int L4 = CW >> 2;                        // float4 lanes per tap
-  const int chunks = Cin / CW;
-  const int co = blockIdx.x / chunks, ci0 = (blockIdx.x - co * chunks) * CW;
   const size_t st4 = (size_t)slice / 4;
   for (int u = threadIdx.x; u < kk * L4; u += 256) {
     const int t = u / L4, lane = u - t * L4;
@@ -972,7 +973,7 @@ extern "C" size_t etb_conv_wgrad_workspace_bytes(const EtbConvParams* cp) {
 extern "C" int etb_conv_wgrad(const void* x_bf16, const void* dy_bf16, float* dw_f32, const EtbConvParams* cp, int32_t flags, void* workspace,
                               size_t workspace_bytes, void* stream) {
   ETB_CHECK_ARG(x_bf16 && dy_bf16 && dw_f32 && cp && workspace);
-  ETB_CHECK_ARG(cp->N > 0 && cp->H > 0 && cp->W > 0 && cp->Cin > 0 && cp->Cout > 0 && cp->Cin % 8 == 0 && (cp->Cin % 64 == 0 || cp->Cin < 64));
+  ETB_CHECK_ARG(cp->N > 0 && cp->H > 0 && cp->W > 0 && cp->Cin > 0 && cp->Cout > 0 && cp->Cin % 8 == 0);
   ETB_CHECK_ARG(cp->kh * cp->kw <= 12 && (cp->stride == 1 || cp->stride == 2));
   ETB_CHECK_ARG(cp->x_cstride % 8 == 0 && cp->y_cstride % 8 == 0 && (((uintptr_t)x_bf16) & 15) == 0 && (((uintptr_t)dy_bf16) & 15) == 0);
   ETB_CHECK_ARG((((uintptr_t)workspace) & 15) == 0);
@@ -1042,7 +1043,7 @@ extern "C" int etb_conv_wgrad(const void* x_bf16, const void* dy_bf16, float* dw
   const long cap = (long)etb_num_sms() * 16;
   if (blocks > cap) blocks = cap;
   if (wa.ntaps > 1 && !(flags & 1))
-    etb_launch(wgrad_reduce_taps_kernel, dim3((unsigned)(cp->Cout * (cp->Cin < 64 ? 1 : cp->Cin >> 6))), dim3(256), 0, st, (const float*)workspace, (long)dw_elems, splitk, dw_f32, cp->Cin, wa.ntaps,
+    etb_launch(wgrad_reduce_taps_kernel, dim3((unsigned)(cp->Cout * ((cp->Cin + 63) >> 6))), dim3(256), 0, st, (const float*)workspace, (long)dw_elems, splitk, dw_f32, cp->Cin, wa.ntaps,
                                                                                   flags);
   else if (splitk >= 32)
     etb_launch(wgrad_reduce_kernel<16>, dim3((unsigned)blocks), dim3(dim3(32, 16)), 0, st, (const float*)workspace, (long)dw_elems, splitk, dw_f32, cp->Cout, cp->Cin, wa.ntaps, flags);

@@ -76,7 +76,9 @@ extern "C" int etb_column_sum(const float* partials, int64_t rows, int32_t C, fl
 
 // ------------------------------------------------------------------------------------------------ netD tail (C -> 2)
 #define NETD_THREADS 256
-#define NETD_MAXG 4          // channel groups of 8 per lane: C <= 32*8*4 = 1024
+// MAXG channel groups of 8 per lane: C <= 32*8*MAXG.  MAXG 4 (C <= 1024) serves YOLOv5n-l; MAXG 5 (C <= 1280) is a
+// second instance for YOLOv5x's det_32, so the narrower layers keep the smaller register allocation.
+#define NETD_MAXG_MAX 5
 __device__ __forceinline__ void bf8_to_f(const uint4 v, float* f) {
   const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&v);
 #pragma unroll
@@ -111,6 +113,7 @@ __global__ void __launch_bounds__(NETD_THREADS) netd_tail_fwd_kernel(const __nv_
 
 // dh[m][c] = (h[m][c] > 0) * (do[m][0]*w2[0][c] + do[m][1]*w2[1][c])   (ReLU mask of relu(conv1) folded in)
 // partial dW2[j][c] = sum over this block's rows of do[m][j] * h[m][c]  -> partials[blockIdx][2][C]
+template <int NETD_MAXG>
 __global__ void __launch_bounds__(NETD_THREADS) netd_tail_bwd_kernel(const float* __restrict__ dout, const __nv_bfloat16* __restrict__ h, long M, int C,
                                                                      int hcs, const float* __restrict__ w2, __nv_bfloat16* __restrict__ dh,
                                                                      float* __restrict__ partials) {
@@ -183,21 +186,28 @@ extern "C" int etb_netd_tail_fwd(const void* h_bf16, int64_t M, int32_t C, int32
   return ETB_OK;
 }
 
-// partials: [etb_netd_tail_rows(M)][2][C] floats (fully overwritten); dW2 = etb_column_sum(partials, rows, 2*C, ...)
-extern "C" int etb_netd_tail_bwd(const float* dout, const void* h_bf16, int64_t M, int32_t C, int32_t h_cstride, const float* w2, void* dh_bf16,
-                                 float* partials, int32_t rows, void* stream) {
-  ETB_CHECK_ARG(dout && h_bf16 && w2 && dh_bf16 && partials && M > 0 && C >= 8 && C % 8 == 0 && C <= 256 * NETD_MAXG);
-  ETB_CHECK_ARG(h_cstride >= C && h_cstride % 8 == 0 && rows == netd_blocks(M));
+template <int MAXG>
+static int launch_netd_tail_bwd(const float* dout, const void* h_bf16, int64_t M, int32_t C, int32_t h_cstride, const float* w2, void* dh_bf16,
+                                float* partials, int32_t rows, cudaStream_t st) {
   const size_t smem = (size_t)(NETD_THREADS / 32) * 2 * C * sizeof(float);
   static bool attr_done = false;
   if (!attr_done) {
-    ETB_CHECK_CUDA(cudaFuncSetAttribute(netd_tail_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (NETD_THREADS / 32) * 2 * 256 * NETD_MAXG * 4));
+    ETB_CHECK_CUDA(cudaFuncSetAttribute(netd_tail_bwd_kernel<MAXG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (NETD_THREADS / 32) * 2 * 256 * MAXG * 4));
     attr_done = true;
   }
-  etb_launch(netd_tail_bwd_kernel, dim3(rows), dim3(NETD_THREADS), smem, (cudaStream_t)stream, dout, (const __nv_bfloat16*)h_bf16, (long)M, C, h_cstride, w2,
-                                                                         (__nv_bfloat16*)dh_bf16, partials);
+  etb_launch(netd_tail_bwd_kernel<MAXG>, dim3(rows), dim3(NETD_THREADS), smem, st, dout, (const __nv_bfloat16*)h_bf16, (long)M, C, h_cstride, w2,
+             (__nv_bfloat16*)dh_bf16, partials);
   ETB_CHECK_LAUNCH();
   return ETB_OK;
+}
+
+// partials: [etb_netd_tail_rows(M)][2][C] floats (fully overwritten); dW2 = etb_column_sum(partials, rows, 2*C, ...)
+extern "C" int etb_netd_tail_bwd(const float* dout, const void* h_bf16, int64_t M, int32_t C, int32_t h_cstride, const float* w2, void* dh_bf16,
+                                 float* partials, int32_t rows, void* stream) {
+  ETB_CHECK_ARG(dout && h_bf16 && w2 && dh_bf16 && partials && M > 0 && C >= 8 && C % 8 == 0 && C <= 256 * NETD_MAXG_MAX);
+  ETB_CHECK_ARG(h_cstride >= C && h_cstride % 8 == 0 && rows == netd_blocks(M));
+  if (C > 1024) return launch_netd_tail_bwd<5>(dout, h_bf16, M, C, h_cstride, w2, dh_bf16, partials, rows, (cudaStream_t)stream);
+  return launch_netd_tail_bwd<4>(dout, h_bf16, M, C, h_cstride, w2, dh_bf16, partials, rows, (cudaStream_t)stream);
 }
 
 // ------------------------------------------------------------------------------------------------ domain focal loss

@@ -98,9 +98,7 @@ class Conv(nn.Module):
     def fused(self, x):
         """True when this Conv runs as ONE ConvBnActFn (and can therefore write into a CatBuf slice / add a shortcut)."""
         c = self.conv.out_channels
-        # csrc/bn.cu (bn_c_ok): one thread owns 8 channels and C/8 must be a power of two <= 256; other widths (YOLOv5m:
-        # 48/96/192/...) run the native conv + torch BatchNorm/activation scaffold below instead of raising
-        bn_ok = c % 8 == 0 and (c // 8) & (c // 8 - 1) == 0 and c // 8 <= 256
+        bn_ok = c % 8 == 0 and c // 8 <= 256       # csrc/bn.cu bn_c_ok: one thread owns 8 channels, C/8 <= 256 per block
         return (Conv.NATIVE and Conv.FUSED_BN and bn_ok and x.is_cuda and self.training
                 and native_act(self.act) is not None)
 
