@@ -11,9 +11,11 @@ reference's DDP without SyncBN; the only collective is one SUM all-reduce of the
 (loss*WORLD_SIZE followed by DDP's mean == sum of per-rank gradients); teachers stay bit-identical on all ranks
 because the reduced gradients are.
 """
+import gc
 import math
 
 import os
+from collections import namedtuple
 
 import numpy as np
 import torch
@@ -34,41 +36,33 @@ def one_cycle(y1=0.0, y2=1.0, steps=100):  # reference utils/general.py:480-482
     return lambda x: ((1 - math.cos(x * math.pi / steps)) / 2) * (y2 - y1) + y1
 
 
-class SSODTrainerStep:
-    def __init__(self, cfg, device, rank=-1, world_size=1, epochs=None, batch_size=None, amp_dtype=torch.bfloat16,
-                 pseudo_label_stats=None, nb=None, start_epoch=0):
-        """pseudo_label_stats (LabelMatch only): dict(target_data_len, label_num_per_image, cls_ratio_gt) that the reference
-        derives from its datasets (ssod_trainer.py:71).  nb = batches per epoch (len(train_loader)); it only sizes the
-        warm-up window exactly like trainer/trainer.py:372-376 (nb=None: the 1000-iteration floor)."""
+# What a captured step is; TrainerStep._graphed / _capture own everything else.  Plain functions of the step:
+#   static(step, key, *inputs) -> dict of static input buffers, filled from the inputs of the capturing call
+#   stage(step, g, *inputs): copy one call's inputs into those buffers (stream-ordered, no host sync)
+#   body(step, g) -> the detached loss: forward + loss + _backward on the static buffers (graph A)
+#   ema_update(step, scalars_dev): the EMA update of graph B, decays read from device memory
+#   ema_decays(step) -> the decays of this optimizer step for ema_scalars(); advances the update counters like .update()
+GraphHooks = namedtuple("GraphHooks", "static stage body ema_update ema_decays")
+
+
+class TrainerStep:
+    """What the SSOD and the supervised step share: optimizer, warm-up / accumulate cadence, gradient arena, all-reduce,
+    the eager optimizer + EMA update, and the capture / replay of a step as two CUDA graphs."""
+
+    fixed_accumulate = False     # trainer/trainer.py has no such switch; the SSOD step reads cfg.SSOD.fixed_accumulate
+
+    def __init__(self, cfg, model, device, rank, world_size, epochs, batch_size, amp_dtype, nb, start_epoch):
         self.cfg, self.device = cfg, device
         self.RANK, self.WORLD_SIZE = rank, world_size
         self.epochs = epochs if epochs is not None else cfg.epochs
         self.epoch = 0
         self.batch_size = batch_size if batch_size is not None else cfg.Dataset.batch_size
         self.amp_dtype = amp_dtype
-        self.model = Model(cfg).to(device)
-        self.model_type = self.model.model_type
-        self.ema = ModelEMA(self.model)
-        if cfg.hyp.burn_epochs > 0:
-            self.semi_ema = None
-        elif cfg.SSOD.cosine_ema:
-            self.semi_ema = CosineEMA(self.ema.ema, decay_start=cfg.SSOD.ema_rate, total_epoch=self.epochs)
-        else:
-            self.semi_ema = SemiSupModelEMA(self.ema.ema, cfg.SSOD.ema_rate)
-        self.fixed_accumulate = cfg.SSOD.fixed_accumulate
+        self.model = model.to(device)
+        self.ema = ModelEMA(self.model)          # the reference keeps it on rank 0/-1 only (trainer.py:157); harmless elsewhere
+        self.semi_ema = None
         self.build_optimizer(cfg)
         self.compute_loss = ComputeLoss(self.model, cfg)
-        self.compute_un_sup_loss = ComputeStudentMatchLoss(self.model, cfg)
-        self.domain_loss, self.target_loss = DomainLoss(), TargetLoss()       # ssod_trainer.py:262-263
-        if getattr(cfg.SSOD, "pseudo_label_type", "FairPseudoLabel") == "LabelMatch":      # ssod_trainer.py:69-71
-            from .labelmatch import LabelMatch
-            ps = pseudo_label_stats or {}
-            nc = cfg.Dataset.nc
-            self.pseudo_label_creator = LabelMatch(cfg, int(ps.get("target_data_len", 0) / max(world_size, 1)), ps.get("label_num_per_image", 7.0),
-                                                   ps.get("cls_ratio_gt", np.full(nc, 1.0 / nc)))
-        else:
-            self.pseudo_label_creator = FairPseudoLabel(cfg)
-        self.da_loss_weights = cfg.SSOD.da_loss_weights
         self.last_opt_step = -1
         # trainer/trainer.py:372-376: number of warm-up iterations = max(warmup_epochs * nb, 1000), capped at half the run
         self.nb = nb
@@ -79,16 +73,11 @@ class SSODTrainerStep:
         else:
             self.nw = -1
         self._arena = None
-        self.last = {}
-        self.profile = False     # record CUDA events at the phase boundaries of train_instance
-        self.phase_events = []
-        self._graph = None       # captured CUDA graph of the whole step (train_instance_graphed)
-        self._ema_scalars_dev = None
-        self._teacher_stream = None
-        self._teacher_keep = None
         self._bn_sync = None
-        self._burn_graph = None     # captured burn-in step (train_without_unlabeled[_da]_graphed)
-        self.burn_in_captures = 0   # how many times a burn-in step has been captured
+        self.last = {}
+        self.profile = False     # record CUDA events at the phase boundaries of the eager step
+        self.phase_events = []
+        self._graph = None       # the step captured as CUDA graphs (see _graphed)
 
     # trainer/trainer.py:193-217
     def build_optimizer(self, cfg):
@@ -119,17 +108,13 @@ class SSODTrainerStep:
             self._arena = GradArena(self.model.parameters(), self.device, reverse=True)   # backward-completion order
         return self._arena
 
-    # "sum" = the reference (loss * WORLD_SIZE, then DDP's mean: trainer/ssod_trainer.py:638-648).  "avg" (ncclAvg: the same
-    # collective at the same cost) is for synthetic benchmarks only: with SUM the effective learning rate grows with the world
-    # size, and a random-init model's BatchNorm scales then drift WORLD_SIZE x faster (bench.py's self-check explains why that
-    # matters); set before the first step.
-    GRAD_REDUCE = os.environ.get("ETB_GRAD_REDUCE", "sum")
-
+    # GRAD_REDUCE and WGRAD_SIDE_STREAM are read from SSODTrainerStep by both steps: callers set them there
+    # (SSODTrainerStep.GRAD_REDUCE = "avg"), and one assignment has to govern the supervised step as well.
     def _allreduce_grads(self):
         """WORLD_SIZE > 1: one all-reduce of the whole gradient arena"""
         if self.WORLD_SIZE <= 1:
             return
-        self._arena.average = (self.GRAD_REDUCE == "avg")
+        self._arena.average = (SSODTrainerStep.GRAD_REDUCE == "avg")
         self._arena.all_reduce_sum(self.WORLD_SIZE)
 
     def _bn_broadcast(self):
@@ -140,15 +125,12 @@ class SSODTrainerStep:
                 self._bn_sync = BnBufferSync(self.model)
             self._bn_sync.broadcast(self.WORLD_SIZE)
 
-    # trainer/ssod_trainer.py:458-488 (bf16 autocast needs no GradScaler; loss scale == 1), in three parts so that the
-    # gradient all-reduce can sit between two captured CUDA graphs when WORLD_SIZE > 1
-    WGRAD_SIDE_STREAM = os.environ.get("ETB_WGRAD_SIDE", "1") == "1"   # ETB_WGRAD_SIDE=0 disables
-    TEACHER_SIDE_STREAM = os.environ.get("ETB_TEACHER_SIDE", "1") == "1"   # teacher forward + NMS concurrent with the student forward
-
+    # trainer/ssod_trainer.py:458-488 (bf16 autocast needs no GradScaler; loss scale == 1), in parts so that the gradient
+    # all-reduce can sit between two captured CUDA graphs when WORLD_SIZE > 1
     def _backward(self, loss):
         self._ensure_arena()
         from . import autograd_conv as ac
-        ac.backward(loss, side=self.WGRAD_SIDE_STREAM)   # weight-gradient branch on a side stream, joined before returning
+        ac.backward(loss, side=SSODTrainerStep.WGRAD_SIDE_STREAM)   # weight-gradient branch on a side stream, joined before returning
         self._mark("backward")
 
     def _warmup(self, ni):
@@ -165,23 +147,24 @@ class SSODTrainerStep:
                     x['momentum'] = float(np.interp(ni, xi, [self.warmup_momentum, self.momentum]))
         return ni - self.last_opt_step >= self.accumulate
 
-    def _step_and_ema(self, capturing=False):
+    def _step_and_ema(self):
         self.optimizer.step(zero_grad=True)      # fused SGD-Nesterov; also performs optimizer.zero_grad() on the arena
         if self.semi_ema:
-            # == ema.update(model); semi_ema.update(ema.ema); inside a captured graph the decays come from device memory
-            update_ema_pair(self.ema, self.semi_ema, self.model, scalars_dev=self._ema_scalars_dev if capturing else None)
+            update_ema_pair(self.ema, self.semi_ema, self.model)   # == ema.update(model); semi_ema.update(ema.ema)
         else:
             self.ema.update(self.model)
 
     def _optimizer_ema(self, ni):
+        # the gradients are reduced only on the iterations that step, like graph B: a SUM all-reduce of an arena that already
+        # holds reduced gradients (accumulate > 1) would count them WORLD_SIZE times
         if self._warmup(ni):
+            self._allreduce_grads()
+            self._mark("allreduce")
             self._step_and_ema()
             self.last_opt_step = ni
 
     def update_optimizer(self, loss, ni):
         self._backward(loss)
-        self._allreduce_grads()
-        self._mark("allreduce")
         self._optimizer_ema(ni)
 
     def _mark(self, name):
@@ -198,6 +181,161 @@ class SSODTrainerStep:
                 out[n1] = out.get(n1, 0.0) + e0.elapsed_time(e1)
         return out
 
+    # the single ModelEMA of the supervised and the burn-in step, as graph B runs it
+    def _ema_update_dev(self, scalars_dev):
+        self.ema._update_with(self.model, 0.0, scalars_dev=scalars_dev)
+
+    def _ema_decays(self):
+        self.ema.updates += 1
+        return (self.ema.decay(self.ema.updates),)
+
+    # ---- the whole step as CUDA graphs ------------------------------------------------------------------------------
+    def _graphed(self, slot, key, hooks, inputs, ni):
+        """The step described by `hooks` (GraphHooks), captured once per `key` and replayed as two graphs: A = forward ...
+        backward (gradients accumulate in the arena), B = SGD-Nesterov + the EMA update(s).  B is replayed on the
+        iterations the reference's cadence steps the optimizer (ssod_trainer.py:462-488: `accumulate`, warm-up); for
+        WORLD_SIZE > 1 the NCCL all-reduce sits between A and B.  The ~1.5k kernel launches + the autograd traversal
+        collapse into two cudaGraphLaunch calls.  Inputs are copied into static buffers; learning rate / momentum (warm-up,
+        scheduler) and the EMA decays of the step are host scalars written to device memory before the replay, so the
+        schedule needs no re-capture.  The graphs and their buffers live in the attribute `slot`; a new key re-captures."""
+        if getattr(self, slot) is None or getattr(self, slot)["key"] != key:
+            setattr(self, slot, None)            # release the old graphs and their memory pool before capturing new ones
+            setattr(self, slot, self._capture(key, hooks, inputs, ni))
+        g = getattr(self, slot)
+        hooks.stage(self, g, *inputs)
+        # everything the host contributes to this iteration is enqueued BEFORE graph A, so that A, the all-reduce and B follow
+        # each other on the stream without a host gap: accumulate / lr / momentum of iteration ni (host scalars), and -- when
+        # the optimizer is due -- the EMA decays and the SGD hyper-parameters (stream-ordered copies: the previous replay of B
+        # has consumed the old values by the time they land)
+        due = self._warmup(ni)
+        if due:
+            # pageable source: the runtime stages the 16 bytes before returning, so the next step cannot overwrite them early
+            g["ema_dev"].copy_(torch.tensor(ema_scalars(*hooks.ema_decays(self)), dtype=torch.float32))
+            self.optimizer.refresh_hyper()   # lr / momentum of this step -> device memory read by the captured SGD kernel
+        self._bn_broadcast()
+        g["graph"].replay()
+        if due:
+            self._allreduce_grads()          # one all-reduce per optimizer step, between the two graphs (enqueued, no host sync)
+            g["graph_b"].replay()
+            self.last_opt_step = ni
+        return g["loss"]
+
+    def _capture(self, key, hooks, inputs, ni):
+        dev = self.device
+        g = hooks.static(self, key, *inputs)
+        g.update(key=key, ema_dev=torch.zeros(4, dtype=torch.float32, device=dev))
+        was_profile, self.profile = self.profile, False
+        self.last = {}
+        restore = self._snapshot_training_state()
+        # warm-up on a side stream (allocator + lazily-created state: momentum buffers, chunk tables, workspaces, TMA/func attrs)
+        side = torch.cuda.Stream(device=dev)
+        side.wait_stream(torch.cuda.current_stream(dev))
+        with torch.cuda.stream(side):
+            for _ in range(2):
+                hooks.body(self, g)
+                self._allreduce_grads()
+                self._warmup(ni)
+                self._step_and_ema()          # the optimizer + EMA branch is exercised (and later captured) unconditionally
+        torch.cuda.current_stream(dev).wait_stream(side)
+        torch.cuda.synchronize(dev)
+        # No cyclic garbage collection while the stream captures: a step that only the collector frees (an SSOD step is in
+        # a reference cycle through its `lf` closure) would destroy its CUDA graphs in the middle of this capture, and
+        # destroying a graph is not permitted while a stream captures: it invalidates the capture.  Dead steps go now.
+        gc.collect()
+        gc_enabled = gc.isenabled()
+        gc.disable()
+        try:
+            graph = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(graph):
+                g["loss"] = hooks.body(self, g)
+            g["graph"] = graph
+            gb = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(gb, pool=graph.pool()):
+                self.optimizer.step(zero_grad=True)
+                hooks.ema_update(self, g["ema_dev"])
+            g["graph_b"] = gb
+        finally:
+            if gc_enabled:
+                gc.enable()
+        restore()
+        self.profile = was_profile
+        return g
+
+    def _snapshot_training_state(self):
+        """The warm-up steps before a capture really train: snapshot every piece of state they touch (weights, BN
+        statistics, the EMA model(s), momentum, the gradients accumulated towards the next optimizer step, the counters,
+        lr / momentum) and return the function that puts it back."""
+        self._ensure_arena()
+        emas = [e for e in (self.ema, self.semi_ema) if e is not None]
+        had_momentum = any(len(self.optimizer.state[p]) for g_ in self.optimizer.param_groups for p in g_["params"])
+        tensors = [t for m in [self.model] + [e.ema for e in emas] for t in m.state_dict().values()]
+        if had_momentum:
+            tensors += [self.optimizer.state[p]["momentum_buffer"] for g_ in self.optimizer.param_groups for p in g_["params"]
+                        if self.optimizer.state[p].get("momentum_buffer") is not None]
+        tensors.append(self._arena.flat)     # gradients already accumulated towards the next optimizer step (accumulate > 1)
+        snap = [t.clone() for t in tensors]
+        saved = (self.last_opt_step, [e.updates for e in emas], self.accumulate,
+                 [(x['lr'], x.get('momentum')) for x in self.optimizer.param_groups])
+
+        def restore():
+            with torch.no_grad():
+                for t, c in zip(tensors, snap):
+                    t.copy_(c)
+                if not had_momentum:      # buffers created by the warm-up: zero == "not yet created" for SGD (buf = grad on first use)
+                    for g_ in self.optimizer.param_groups:
+                        for p in g_["params"]:
+                            b = self.optimizer.state[p].get("momentum_buffer")
+                            if b is not None:
+                                b.zero_()
+            self.last_opt_step, updates, self.accumulate, hyp = saved
+            for e, u in zip(emas, updates):
+                e.updates = u
+            for x, (lr, mom) in zip(self.optimizer.param_groups, hyp):
+                x['lr'] = lr
+                if mom is not None:
+                    x['momentum'] = mom
+        return restore
+
+
+class SSODTrainerStep(TrainerStep):
+    def __init__(self, cfg, device, rank=-1, world_size=1, epochs=None, batch_size=None, amp_dtype=torch.bfloat16,
+                 pseudo_label_stats=None, nb=None, start_epoch=0):
+        """pseudo_label_stats (LabelMatch only): dict(target_data_len, label_num_per_image, cls_ratio_gt) that the reference
+        derives from its datasets (ssod_trainer.py:71).  nb = batches per epoch (len(train_loader)); it only sizes the
+        warm-up window exactly like trainer/trainer.py:372-376 (nb=None: the 1000-iteration floor)."""
+        super().__init__(cfg, Model(cfg), device, rank, world_size, epochs, batch_size, amp_dtype, nb, start_epoch)
+        self.model_type = self.model.model_type
+        if cfg.hyp.burn_epochs > 0:
+            self.semi_ema = None
+        elif cfg.SSOD.cosine_ema:
+            self.semi_ema = CosineEMA(self.ema.ema, decay_start=cfg.SSOD.ema_rate, total_epoch=self.epochs)
+        else:
+            self.semi_ema = SemiSupModelEMA(self.ema.ema, cfg.SSOD.ema_rate)
+        self.fixed_accumulate = cfg.SSOD.fixed_accumulate
+        self.compute_un_sup_loss = ComputeStudentMatchLoss(self.model, cfg)
+        self.domain_loss, self.target_loss = DomainLoss(), TargetLoss()       # ssod_trainer.py:262-263
+        if getattr(cfg.SSOD, "pseudo_label_type", "FairPseudoLabel") == "LabelMatch":      # ssod_trainer.py:69-71
+            from .labelmatch import LabelMatch
+            ps = pseudo_label_stats or {}
+            nc = cfg.Dataset.nc
+            self.pseudo_label_creator = LabelMatch(cfg, int(ps.get("target_data_len", 0) / max(world_size, 1)), ps.get("label_num_per_image", 7.0),
+                                                   ps.get("cls_ratio_gt", np.full(nc, 1.0 / nc)))
+        else:
+            self.pseudo_label_creator = FairPseudoLabel(cfg)
+        self.da_loss_weights = cfg.SSOD.da_loss_weights
+        self._teacher_stream = None
+        self._teacher_keep = None
+        self._burn_graph = None     # captured burn-in step (train_without_unlabeled[_da]_graphed)
+        self.burn_in_captures = 0   # how many times a burn-in step has been captured
+
+    # "sum" = the reference (loss * WORLD_SIZE, then DDP's mean: trainer/ssod_trainer.py:638-648).  "avg" (ncclAvg: the same
+    # collective at the same cost) is for synthetic benchmarks only: with SUM the effective learning rate grows with the world
+    # size, and a random-init model's BatchNorm scales then drift WORLD_SIZE x faster (bench.py's self-check explains why that
+    # matters); set before the first step.  Governs the supervised step too.
+    GRAD_REDUCE = os.environ.get("ETB_GRAD_REDUCE", "sum")
+    WGRAD_SIDE_STREAM = os.environ.get("ETB_WGRAD_SIDE", "1") == "1"   # ETB_WGRAD_SIDE=0 disables; governs the supervised step too
+    TEACHER_SIDE_STREAM = os.environ.get("ETB_TEACHER_SIDE", "1") == "1"   # teacher forward + NMS concurrent with the student forward
+
     def split_predict_and_feature(self, total_pred, total_feature, n_img):
         """ssod_trainer.py:568-585.  split_batch == t[:n], t[n:] whose backward is a no-op (the loss kernels write both
         gradients into one buffer) instead of autograd's zeros + copy + add per slice."""
@@ -213,7 +351,7 @@ class SSODTrainerStep:
         n_img = imgs.shape[0]
         self._mark("start")
         if self.WORLD_SIZE > 1 and not torch.cuda.is_current_stream_capturing():
-            self._bn_broadcast()         # (captured steps: train_instance_graphed issues it before the replay)
+            self._bn_broadcast()         # (captured steps: _graphed issues it before the replay)
         # The teacher forward + NMS + pseudo-label transform feed nothing but the unsupervised loss, and the student forward
         # does not depend on them: with the device-resident pseudo labels they run on a side stream, concurrently with the
         # student forward (the teacher's batch-16 kernels leave SMs idle on the deep, small maps; the student's fill them),
@@ -285,46 +423,47 @@ class SSODTrainerStep:
         return loss.detach()
 
     # ---- the whole step as CUDA graphs ------------------------------------------------------------------------------
-    def train_instance_graphed(self, imgs, targets, unlabeled_imgs, unlabeled_imgs_ori, unlabeled_gt, unlabeled_M, ni):
-        """train_instance captured once (static shapes, device-resident pseudo labels, no host sync anywhere in the step)
-        and replayed as two graphs: A = teacher forward ... backward (gradients accumulate in the arena), B = SGD-Nesterov +
-        both EMA updates.  B is replayed on the iterations the reference's cadence steps the optimizer
-        (ssod_trainer.py:462-488: `accumulate`, warm-up); for WORLD_SIZE > 1 the NCCL all-reduce sits between A and B.  The
-        ~1.5k kernel launches + the autograd traversal collapse into two cudaGraphLaunch calls.  Inputs are copied into
-        static buffers; learning rate / momentum (warm-up, scheduler) and the EMA decays of the step are host scalars
-        written to device memory before B is replayed, so the schedule needs no re-capture."""
-        self._require_semi_ema()
-        shapes = (tuple(imgs.shape), tuple(targets.shape), tuple(unlabeled_imgs.shape), tuple(unlabeled_M.shape),
-                  imgs.dtype, unlabeled_imgs.dtype, unlabeled_imgs_ori.dtype)      # uint8 loader batches vs fp32: different static buffers
-        if self._graph is not None and self._graph["shapes"] != shapes:
-            self.reset_graph()
-        if self._graph is None:
-            self._capture(imgs, targets, unlabeled_imgs, unlabeled_imgs_ori, unlabeled_M, ni, shapes)
-        g = self._graph
+    def _ssod_static(self, key, imgs, targets, us, uw, Ms):
+        return dict(imgs=imgs.clone(), targets=targets.clone(), us=us.clone(), uw=uw.clone(), Ms=Ms.to(self.device, torch.float64).clone())
+
+    def _ssod_stage(self, g, imgs, targets, us, uw, Ms):
         g["imgs"].copy_(imgs, non_blocking=True)
         g["targets"].copy_(targets, non_blocking=True)
-        g["us"].copy_(unlabeled_imgs, non_blocking=True)
-        g["uw"].copy_(unlabeled_imgs_ori, non_blocking=True)
-        g["Ms"].copy_(unlabeled_M, non_blocking=True)
-        # everything the host contributes to this iteration is enqueued BEFORE graph A, so that A, the all-reduce and B follow
-        # each other on the stream without a host gap: accumulate / lr / momentum of iteration ni (host scalars), and -- when
-        # the optimizer is due -- the EMA decays and the SGD hyper-parameters (stream-ordered copies: the previous replay of B
-        # has consumed the old values by the time they land)
-        due = self._warmup(ni)
-        if due:
-            d1, d2 = next_pair_decays(self.ema, self.semi_ema)
-            # pageable source: the runtime stages the 16 bytes before returning, so the next step cannot overwrite them early
-            self._ema_scalars_dev.copy_(torch.tensor(ema_scalars(d1, d2), dtype=torch.float32))
-            self.optimizer.refresh_hyper()   # lr / momentum of this step -> device memory read by the captured SGD kernel
-        self._bn_broadcast()
-        g["graph"].replay()
-        if due:
-            self._allreduce_grads()          # one SUM all-reduce per optimizer step, between the two graphs (enqueued, no host sync)
-            g["graph_b"].replay()
-            self.last_opt_step = ni
+        g["us"].copy_(us, non_blocking=True)
+        g["uw"].copy_(uw, non_blocking=True)
+        g["Ms"].copy_(Ms, non_blocking=True)
+
+    def _ssod_body(self, g):
+        return self.train_instance(g["imgs"], g["targets"], g["us"], g["uw"], None, g["Ms"], None, _stop_after_backward=True)
+
+    _SSOD_GRAPH = GraphHooks(_ssod_static, _ssod_stage, _ssod_body,
+                             lambda self, scalars_dev: update_ema_pair(self.ema, self.semi_ema, self.model, scalars_dev=scalars_dev),
+                             lambda self: next_pair_decays(self.ema, self.semi_ema))
+
+    def train_instance_graphed(self, imgs, targets, unlabeled_imgs, unlabeled_imgs_ori, unlabeled_gt, unlabeled_M, ni):
+        """train_instance captured once (static shapes, device-resident pseudo labels, no host sync anywhere in the step)
+        and replayed as two graphs (TrainerStep._graphed): A = teacher forward ... backward, B = SGD-Nesterov + both EMA
+        updates."""
+        self._require_semi_ema()
+        key = (tuple(imgs.shape), tuple(targets.shape), tuple(unlabeled_imgs.shape), tuple(unlabeled_M.shape),
+               imgs.dtype, unlabeled_imgs.dtype, unlabeled_imgs_ori.dtype)      # uint8 loader batches vs fp32: different static buffers
+        loss = self._graphed("_graph", key, self._SSOD_GRAPH, (imgs, targets, unlabeled_imgs, unlabeled_imgs_ori, unlabeled_M), ni)
         if hasattr(self.pseudo_label_creator, "stage_detections"):   # LabelMatch: the captured step cannot stage its detections itself
             self.pseudo_label_creator.stage_detections()
-        return g["loss"]
+        return loss
+
+    def _snapshot_training_state(self):
+        """+ the LabelMatch image counters, which the SSOD warm-up steps before a capture advance"""
+        restore = super()._snapshot_training_state()
+        c = self.pseudo_label_creator
+        if not hasattr(c, "count"):
+            return restore
+        counts = (c.count, c.pse_count)
+
+        def restore_with_counts():
+            restore()
+            c.count, c.pse_count = counts
+        return restore_with_counts
 
     def after_epoch(self, epoch, start_epoch=0):
         """ssod_trainer.py:319-323: LabelMatch re-estimates the per-class thresholds once per epoch; the unsupervised loss
@@ -338,78 +477,6 @@ class SSODTrainerStep:
 
     def reset_graph(self):
         self._graph = None
-        self._ema_scalars_dev = None
-
-    def _capture(self, imgs, targets, us, uw, Ms, ni, shapes):
-        dev = self.device
-        st = dict(shapes=shapes, imgs=imgs.clone(), targets=targets.clone(), us=us.clone(), uw=uw.clone(),
-                  Ms=Ms.to(dev, torch.float64).clone())
-        self._ema_scalars_dev = torch.zeros(4, dtype=torch.float32, device=dev)
-        was_profile, self.profile = self.profile, False
-        self.last = {}
-        restore = self._snapshot_training_state()
-        lm_state = None
-        if hasattr(self.pseudo_label_creator, "count"):
-            lm_state = (self.pseudo_label_creator.count, self.pseudo_label_creator.pse_count)
-        # warm-up on a side stream (allocator + lazily-created state: momentum buffers, chunk tables, workspaces, TMA/func attrs)
-        side = torch.cuda.Stream(device=dev)
-        side.wait_stream(torch.cuda.current_stream(dev))
-        with torch.cuda.stream(side):
-            for _ in range(2):
-                self.train_instance(st["imgs"], st["targets"], st["us"], st["uw"], None, st["Ms"], ni, _stop_after_backward=True)
-                self._allreduce_grads()
-                self._warmup(ni)
-                self._step_and_ema()          # the optimizer + EMA branch is exercised (and later captured) unconditionally
-        torch.cuda.current_stream(dev).wait_stream(side)
-        torch.cuda.synchronize(dev)
-        graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(graph):
-            st["loss"] = self.train_instance(st["imgs"], st["targets"], st["us"], st["uw"], None, st["Ms"], ni, _stop_after_backward=True)
-        st["graph"] = graph
-        gb = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(gb, pool=graph.pool()):
-            self._step_and_ema(capturing=True)
-        st["graph_b"] = gb
-        restore()
-        if lm_state is not None:
-            self.pseudo_label_creator.count, self.pseudo_label_creator.pse_count = lm_state
-        self.profile = was_profile
-        self._graph = st
-
-    def _snapshot_training_state(self):
-        """The warm-up steps before a capture really train: snapshot every piece of state they touch (weights, BN
-        statistics, the EMA model(s), momentum, the gradients accumulated towards the next optimizer step, the counters,
-        lr / momentum) and return the function that puts it back."""
-        self._ensure_arena()
-        emas = [e for e in (self.ema, self.semi_ema) if e is not None]
-        had_momentum = any(len(self.optimizer.state[p]) for g_ in self.optimizer.param_groups for p in g_["params"])
-        tensors = [t for m in [self.model] + [e.ema for e in emas] for t in m.state_dict().values()]
-        if had_momentum:
-            tensors += [self.optimizer.state[p]["momentum_buffer"] for g_ in self.optimizer.param_groups for p in g_["params"]
-                        if self.optimizer.state[p].get("momentum_buffer") is not None]
-        tensors.append(self._arena.flat)     # gradients already accumulated towards the next optimizer step (accumulate > 1)
-        snap = [t.clone() for t in tensors]
-        saved = (self.last_opt_step, [e.updates for e in emas], self.accumulate,
-                 [(x['lr'], x.get('momentum')) for x in self.optimizer.param_groups])
-
-        def restore():
-            with torch.no_grad():
-                for t, c in zip(tensors, snap):
-                    t.copy_(c)
-                if not had_momentum:      # buffers created by the warm-up: zero == "not yet created" for SGD (buf = grad on first use)
-                    for g_ in self.optimizer.param_groups:
-                        for p in g_["params"]:
-                            b = self.optimizer.state[p].get("momentum_buffer")
-                            if b is not None:
-                                b.zero_()
-            self.last_opt_step, updates, self.accumulate, hyp = saved
-            for e, u in zip(emas, updates):
-                e.updates = u
-            for x, (lr, mom) in zip(self.optimizer.param_groups, hyp):
-                x['lr'] = lr
-                if mom is not None:
-                    x['momentum'] = mom
-        return restore
 
     # ---- burn-in: trainer/ssod_trainer.py:295-317 (train_in_epoch), :421-456 / :490-533 -----------------------------
     @property
@@ -444,7 +511,7 @@ class SSODTrainerStep:
         """Forward + loss of the burn-in step (the reference computes it under autocast; the fused loss kernels read fp32).
         unlabeled_imgs_ori=None: train_without_unlabeled (:427-443), else train_without_unlabeled_da (:498-520)."""
         if self.WORLD_SIZE > 1 and not torch.cuda.is_current_stream_capturing():
-            self._bn_broadcast()         # (captured steps: _burn_in_graphed issues it before the replay)
+            self._bn_broadcast()         # (captured steps: _graphed issues it before the replay)
         with torch.autocast("cuda", dtype=self.amp_dtype):
             # the native stem reads uint8 or fp32 batches in place; with two batches the cat is never materialised
             pred, feats = self.model(imgs if unlabeled_imgs_ori is None else [imgs, unlabeled_imgs_ori])
@@ -487,86 +554,49 @@ class SSODTrainerStep:
     BURN_IN_LABEL_CAPACITY = 64       # initial label capacity of a burn-in graph; doubles when a batch has more labels
 
     def _burn_in_graphed(self, imgs, targets, uw, ni):
-        """The burn-in step as two graphs, like train_instance_graphed: A = forward + loss + backward, [all-reduce], B =
+        """The burn-in step as two graphs (TrainerStep._graphed): A = forward + loss + backward, [all-reduce], B =
         SGD-Nesterov + the single EMA update with its decay read from device memory.  The labels are copied into a static
         buffer of capacity C and their count into a device int32 (stream-ordered, no host sync) that the assigner reads,
         so one capture serves every batch of a given image shape and dtype whatever its label count; a batch with more
         than C labels re-captures with C doubled until it fits."""
         if self.semi_ema is not None:
             raise RuntimeError("burn-in step requested after the hand-over to the semi-supervised phase (semi_ema exists)")
-        nt = int(targets.shape[0])
-        key = (tuple(imgs.shape), imgs.dtype, None if uw is None else (tuple(uw.shape), uw.dtype))
-        g = self._burn_graph
-        cap = self.BURN_IN_LABEL_CAPACITY if g is None else g["cap"]
-        while cap < nt:
+        cap = self.BURN_IN_LABEL_CAPACITY if self._burn_graph is None else self._burn_graph["cap"]
+        while cap < targets.shape[0]:
             cap *= 2
-        if g is None or g["key"] != key or g["cap"] != cap:
-            self._burn_graph = None
-            g = self._capture_burn_in(imgs, targets, uw, ni, key, cap)
+        key = (tuple(imgs.shape), imgs.dtype, None if uw is None else (tuple(uw.shape), uw.dtype), cap)
+        return self._graphed("_burn_graph", key, self._BURN_IN_GRAPH, (imgs, targets, uw), ni)
+
+    def _burn_in_static(self, key, imgs, targets, uw):
+        cap, nt = key[-1], int(targets.shape[0])
+        g = dict(cap=cap, imgs=imgs.clone(), uw=None if uw is None else uw.clone(),
+                 targets=torch.zeros((cap, 6), dtype=torch.float32, device=self.device),
+                 nt=torch.full((1,), nt, dtype=torch.int32, device=self.device))
+        g["targets"][:nt].copy_(targets)
+        self.burn_in_captures += 1
+        return g
+
+    def _burn_in_stage(self, g, imgs, targets, uw):
+        nt = int(targets.shape[0])
         g["imgs"].copy_(imgs, non_blocking=True)
         if uw is not None:
             g["uw"].copy_(uw, non_blocking=True)
         g["targets"][:nt].copy_(targets, non_blocking=True)
-        # pageable sources: the runtime stages these few bytes before returning, so the next step cannot overwrite them early
+        # pageable source: the runtime stages these few bytes before returning, so the next step cannot overwrite them early
         g["nt"].copy_(torch.tensor([nt], dtype=torch.int32))
-        due = self._warmup(ni)
-        if due:
-            self.ema.updates += 1
-            g["ema_dev"].copy_(torch.tensor(ema_scalars(self.ema.decay(self.ema.updates)), dtype=torch.float32))
-            self.optimizer.refresh_hyper()
-        self._bn_broadcast()
-        g["graph"].replay()
-        if due:
-            self._allreduce_grads()
-            g["graph_b"].replay()
-            self.last_opt_step = ni
-        return g["loss"]
 
-    def _burn_in_forward_backward(self, st):
+    def _burn_in_forward_backward(self, g):
         # returns the loss detached: nothing may keep this step's autograd graph alive, because the AccumulateGrad nodes of
         # the parameters it holds are tied to the stream they were created on (the warm-up's side stream, the capture's)
-        loss, _ = self._burn_in_loss(st["imgs"], st["targets"], st["uw"], st["nt"])
+        loss, _ = self._burn_in_loss(g["imgs"], g["targets"], g["uw"], g["nt"])
         self._backward(loss)
         return loss.detach()
 
-    def _capture_burn_in(self, imgs, targets, uw, ni, key, cap):
-        dev = self.device
-        nt = int(targets.shape[0])
-        st = dict(key=key, cap=cap, imgs=imgs.clone(), uw=None if uw is None else uw.clone(),
-                  targets=torch.zeros((cap, 6), dtype=torch.float32, device=dev),
-                  nt=torch.full((1,), nt, dtype=torch.int32, device=dev),
-                  ema_dev=torch.zeros(4, dtype=torch.float32, device=dev))
-        st["targets"][:nt].copy_(targets)
-        was_profile, self.profile = self.profile, False
-        self.last = {}
-        restore = self._snapshot_training_state()
-        side = torch.cuda.Stream(device=dev)
-        side.wait_stream(torch.cuda.current_stream(dev))
-        with torch.cuda.stream(side):
-            for _ in range(2):
-                self._burn_in_forward_backward(st)
-                self._allreduce_grads()
-                self._warmup(ni)
-                self._step_and_ema()
-        torch.cuda.current_stream(dev).wait_stream(side)
-        torch.cuda.synchronize(dev)
-        graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(graph):
-            st["loss"] = self._burn_in_forward_backward(st)
-        st["graph"] = graph
-        gb = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(gb, pool=graph.pool()):
-            self.optimizer.step(zero_grad=True)
-            self.ema._update_with(self.model, 0.0, scalars_dev=st["ema_dev"])
-        st["graph_b"] = gb
-        restore()
-        self.profile = was_profile
-        self.burn_in_captures += 1
-        self._burn_graph = st
-        return st
+    _BURN_IN_GRAPH = GraphHooks(_burn_in_static, _burn_in_stage, _burn_in_forward_backward,
+                                TrainerStep._ema_update_dev, TrainerStep._ema_decays)
 
 
-class SupTrainerStep:
+class SupTrainerStep(TrainerStep):
     """The supervised step (trainer/trainer.py:406-443 train_in_epoch body + :381-404 update_optimizer), BASELINE configs
     #1/#2: student forward -> ComputeLoss -> backward -> [all-reduce] -> SGD-Nesterov -> ModelEMA.update, same native
     kernels as the SSOD step minus the teacher / pseudo-label path.  The optimizer cadence is the reference's:
@@ -575,92 +605,40 @@ class SupTrainerStep:
 
     def __init__(self, cfg, device, rank=-1, world_size=1, epochs=None, batch_size=None, amp_dtype=torch.bfloat16, nb=None,
                  start_epoch=0):
-        self.cfg, self.device = cfg, device
-        self.RANK, self.WORLD_SIZE = rank, world_size
-        self.epochs = epochs if epochs is not None else cfg.epochs
-        self.epoch = 0
-        self.batch_size = batch_size if batch_size is not None else cfg.Dataset.batch_size
-        self.amp_dtype = amp_dtype
-        self.model = SupModel(cfg).to(device)
-        self.ema = ModelEMA(self.model)          # the reference keeps it on rank 0/-1 only (trainer.py:157); harmless elsewhere
-        self.semi_ema = None
-        self.fixed_accumulate = False            # trainer/trainer.py has no such switch
-        SSODTrainerStep.build_optimizer(self, cfg)
-        self.compute_loss = ComputeLoss(self.model, cfg)
-        self._arena = None
-        self.last_opt_step = -1
-        if cfg.hyp.warmup_epochs > 0:
-            self.nw = max(round(cfg.hyp.warmup_epochs * (nb or 0)), 1000)
-            if nb:
-                self.nw = min(self.nw, (self.epochs - start_epoch) / 2 * nb)
-        else:
-            self.nw = -1
-        self._graph = None
+        super().__init__(cfg, SupModel(cfg), device, rank, world_size, epochs, batch_size, amp_dtype, nb, start_epoch)
 
-    _warmup = SSODTrainerStep._warmup
-    _ensure_arena = SSODTrainerStep._ensure_arena
-    _bn_broadcast = SSODTrainerStep._bn_broadcast
-    _bn_sync = None
-
-    def _forward_backward(self, imgs, targets):
+    def _loss(self, imgs, targets):
         if self.WORLD_SIZE > 1 and not torch.cuda.is_current_stream_capturing():
-            self._bn_broadcast()      # DDP broadcast_buffers=True (captured steps: issued before the replay)
+            self._bn_broadcast()      # DDP broadcast_buffers=True (captured steps: _graphed issues it before the replay)
         with torch.autocast("cuda", dtype=self.amp_dtype):
             pred = self.model(imgs)
-        loss, loss_items = self.compute_loss(pred, targets)
-        self._ensure_arena()
-        from . import autograd_conv as ac
-        ac.backward(loss, side=SSODTrainerStep.WGRAD_SIDE_STREAM)
-        return loss.detach()
-
-    def _step_and_ema(self):
-        self.optimizer.step(zero_grad=True)
-        self.ema.update(self.model)
-
-    def train_step(self, imgs, targets, ni):
-        loss = self._forward_backward(imgs, targets)
-        if self._warmup(ni):
-            self._arena.average = (SSODTrainerStep.GRAD_REDUCE == "avg")
-            self._arena.all_reduce_sum(self.WORLD_SIZE)
-            self._step_and_ema()
-            self.last_opt_step = ni
+        loss, _ = self.compute_loss(pred, targets)
         return loss
 
-    def train_step_graphed(self, imgs, targets, ni):
-        """train_step with forward + loss + backward replayed from one captured CUDA graph (static shapes); the optimizer /
-        EMA launches (2 kernels, host-side decay) stay eager on the iterations the cadence asks for."""
-        shapes = (tuple(imgs.shape), tuple(targets.shape), imgs.dtype)
-        if self._graph is None or self._graph["shapes"] != shapes:
-            self._ensure_arena()
-            st = dict(shapes=shapes, imgs=imgs.clone(), targets=targets.clone())
-            tensors = [t for t in self.model.state_dict().values()] + [self._arena.flat]
-            snap = [t.clone() for t in tensors]
-            side = torch.cuda.Stream(device=self.device)
-            side.wait_stream(torch.cuda.current_stream(self.device))
-            with torch.cuda.stream(side):
-                for _ in range(2):
-                    self._forward_backward(st["imgs"], st["targets"])
-            torch.cuda.current_stream(self.device).wait_stream(side)
-            torch.cuda.synchronize(self.device)
-            graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(graph):
-                st["loss"] = self._forward_backward(st["imgs"], st["targets"])
-            st["graph"] = graph
-            with torch.no_grad():
-                for t, c in zip(tensors, snap):       # BN running statistics / num_batches_tracked / the arena
-                    t.copy_(c)
-            self._graph = st
-        g = self._graph
+    def train_step(self, imgs, targets, ni):
+        loss = self._loss(imgs, targets)
+        self.update_optimizer(loss, ni)
+        return loss.detach()
+
+    def _static(self, key, imgs, targets):
+        return dict(imgs=imgs.clone(), targets=targets.clone())
+
+    def _stage(self, g, imgs, targets):
         g["imgs"].copy_(imgs, non_blocking=True)
         g["targets"].copy_(targets, non_blocking=True)
-        self._bn_broadcast()
-        g["graph"].replay()
-        if self._warmup(ni):
-            self._arena.average = (SSODTrainerStep.GRAD_REDUCE == "avg")
-            self._arena.all_reduce_sum(self.WORLD_SIZE)
-            self._step_and_ema()
-            self.last_opt_step = ni
-        return g["loss"]
+
+    def _forward_backward(self, g):
+        loss = self._loss(g["imgs"], g["targets"])
+        self._backward(loss)
+        return loss.detach()
+
+    _GRAPH = GraphHooks(_static, _stage, _forward_backward, TrainerStep._ema_update_dev, TrainerStep._ema_decays)
+
+    def train_step_graphed(self, imgs, targets, ni):
+        """train_step replayed from two captured CUDA graphs (TrainerStep._graphed, static shapes): A = forward + loss +
+        backward, B = SGD-Nesterov + the ModelEMA update with its decay read from device memory."""
+        key = (tuple(imgs.shape), tuple(targets.shape), imgs.dtype)
+        return self._graphed("_graph", key, self._GRAPH, (imgs, targets), ni)
 
 
 class DevicePrefetcher:
