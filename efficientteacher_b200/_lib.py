@@ -102,6 +102,7 @@ _SIGS = {
     "etb_select_targets": (C.c_int, [vp, vp, C.c_int32, C.c_int32, vp, vp, C.c_int32, C.c_int32, vp, vp, vp]),
     "etb_build_targets": (C.c_int, [vp, vp, C.c_int32, C.c_int32, C.POINTER(EtbAssignLevels),
                                     C.POINTER(EtbAssignOut), vp]),
+    "etb_label_class_hist": (C.c_int, [vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp, vp]),
     "etb_bbox_ciou": (C.c_int, [vp, vp, C.c_int32, vp, vp]),
     "etb_loss_workspace_bytes": (C.c_size_t, [C.POINTER(EtbLossParams), C.c_int32]),
     "etb_loss_forward": (C.c_int, [C.POINTER(vp), C.POINTER(EtbLossParams), C.POINTER(EtbAssignOut), vp, vp,

@@ -180,3 +180,34 @@ extern "C" int etb_build_targets(const float* targets, const int32_t* nt_dev, in
   ETB_CHECK_LAUNCH();
   return ETB_OK;
 }
+
+// ---------------------------------------------------------------------------------------------------
+// label_class_hist.  LabelMatch.update's `cls_tmp[int(l[1:2])] += 1` over the labeled rows (reference
+// utils/labelmatch.py:126-134), accumulated into hist[nc+1] on the device.  n = *n_dev (or n_host), clamped to cap;
+// rows at or past n are never read.  int() truncates toward zero, so (-1, nc) is a valid class; anything else
+// (NaN included) is counted in hist[nc].  Integer atomics: the result does not depend on the order.
+// ---------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) label_class_hist_kernel(const float* __restrict__ targets, const int32_t* __restrict__ n_dev,
+                                                               int32_t n_host, int32_t cap, int32_t tstride, int32_t nc,
+                                                               int32_t* __restrict__ hist) {
+  int n = n_dev ? *n_dev : n_host;
+  if (n > cap) n = cap;
+  for (int r = blockIdx.x * blockDim.x + threadIdx.x; r < n; r += gridDim.x * blockDim.x) {
+    const float v = targets[(size_t)r * tstride + 1];
+    const int c = (v > -1.0f && v < (float)nc) ? (int)v : nc;
+    atomicAdd(hist + c, 1);
+  }
+}
+
+extern "C" int etb_label_class_hist(const float* targets, const int32_t* n_dev, int32_t n_host, int32_t cap, int32_t tstride,
+                                    int32_t nc, int32_t* hist, void* stream) {
+  ETB_CHECK_ARG(hist && nc > 0 && tstride >= 2 && cap >= 0 && n_host >= 0 && n_host <= cap);
+  ETB_CHECK_ARG(targets != nullptr || cap == 0);
+  if (cap == 0) return ETB_OK;
+  // grid sized by the capacity (the count may only be known on the device): one launch shape per buffer, so it can be captured
+  const int blocks = (cap + 255) / 256 < 32 ? (cap + 255) / 256 : 32;
+  etb_launch(label_class_hist_kernel, dim3(blocks), dim3(256), 0, (cudaStream_t)stream, targets, n_dev, n_host, cap, tstride, nc,
+             hist);
+  ETB_CHECK_LAUNCH();
+  return ETB_OK;
+}

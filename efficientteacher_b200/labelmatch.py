@@ -11,9 +11,12 @@ running mean number of boxes per epoch), high = a 2-component Gaussian-mixture s
 
 The detections are copied device -> pinned host asynchronously and folded into the lists lazily (flush()), so the training
 step itself still never waits on the host."""
+import ctypes as C
+
 import numpy as np
 import torch
 
+from . import _lib
 from .pseudo_label import FairPseudoLabel
 
 
@@ -36,6 +39,7 @@ class LabelMatch(FairPseudoLabel):
         self.count = 0
         self.pse_count = 0
         self._pending = []          # (det pinned [B,max_det,8], det_cnt pinned [B], event) not yet folded into the lists
+        self._hist = None           # int32 [nc + 1] device class histogram of the labeled targets (class_hist())
 
     # ---- per step -------------------------------------------------------------------------------------------------
     def record_detections(self, det, det_cnt):
@@ -65,21 +69,40 @@ class LabelMatch(FairPseudoLabel):
         ev.record(torch.cuda.current_stream(det.device))
         self._pending.append((h_det, h_cnt, ev))
 
-    def update_device(self, targets):
-        """`update(targets, n_img, n_pse_img)` without a host sync: the class histogram of the labeled targets [n,6] is
-        accumulated on the device and folded into cls_tmp by flush()"""
-        h = torch.bincount(targets[:, 1].long(), minlength=self.nc)[:self.nc]
-        self._cls_dev = h if getattr(self, "_cls_dev", None) is None else self._cls_dev + h
+    def class_hist(self, device):
+        """the device accumulator of update_device: int32 [nc + 1], the last slot counting classes outside [0, nc);
+        allocated once, so a captured step adds into the same memory on every replay"""
+        if self._hist is None:
+            self._hist = torch.zeros(self.nc + 1, dtype=torch.int32, device=device)
+        return self._hist
+
+    def update_device(self, targets, n_dev=None):
+        """`update(targets, n_img, n_pse_img)`'s class histogram without a host sync (etb_label_class_hist): the classes
+        of the labeled targets [n,6] are added into class_hist() and folded into cls_tmp by flush().  n_dev (int32[1]
+        CUDA): targets is a buffer whose first n_dev rows are the labels; the rows past them are not counted."""
+        t = targets if targets.is_cuda else targets.to(torch.cuda.current_device())
+        t = t.float().contiguous()
+        _lib.require_cuda(t, n_dev)
+        hist = self.class_hist(t.device)
+        cap = int(t.shape[0])
+        _lib.check(_lib.lib().etb_label_class_hist(_lib.ptr(t) if cap else C.c_void_p(0), _lib.ptr(n_dev),
+                                                   0 if n_dev is not None else cap, cap, int(t.shape[1]), self.nc,
+                                                   _lib.ptr(hist), _lib.stream_ptr(t.device)), "etb_label_class_hist")
 
     def flush(self):
-        """fold every finished device->host copy into the epoch's score lists (in step order)"""
+        """fold every finished device->host copy into the epoch's score lists (in step order), and the device class
+        histogram into cls_tmp (the accumulator is zeroed, stream-ordered).  A labeled class outside [0, nc) raises
+        IndexError, as the reference's `cls_tmp[int(l[1:2])] += 1` does."""
         for h_det, h_cnt, ev in self._pending:
             ev.synchronize()
             self.record_detections(h_det.numpy(), h_cnt.numpy())
         self._pending = []
-        if getattr(self, "_cls_dev", None) is not None:
-            self.cls_tmp += self._cls_dev.cpu().numpy()
-            self._cls_dev = None
+        if self._hist is not None:
+            h = self._hist.cpu().numpy()
+            self._hist.zero_()
+            if h[self.nc]:
+                raise IndexError("LabelMatch: %d labeled target(s) with a class outside [0, %d)" % (int(h[self.nc]), self.nc))
+            self.cls_tmp += h[:self.nc]
 
     def update(self, labels, n=1, pse_n=1):
         """labelmatch.py:114-124: image / pseudo-label counters and the per-class histogram of the rows handed to the loss"""

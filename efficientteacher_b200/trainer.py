@@ -78,6 +78,7 @@ class TrainerStep:
         self.profile = False     # record CUDA events at the phase boundaries of the eager step
         self.phase_events = []
         self._graph = None       # the step captured as CUDA graphs (see _graphed)
+        self.captures = 0        # how many times _graph has been captured (train_instance_graphed / train_step_graphed)
 
     # trainer/trainer.py:193-217
     def build_optimizer(self, cfg):
@@ -188,6 +189,32 @@ class TrainerStep:
     def _ema_decays(self):
         self.ema.updates += 1
         return (self.ema.decay(self.ema.updates),)
+
+    # ---- the labels of a captured step: a static buffer of capacity C and the count in a device int32 -----------------
+    LABEL_CAPACITY = 64      # initial label capacity of a captured SSOD / supervised step; doubles when a batch has more labels
+
+    def _label_capacity(self, slot, targets, initial):
+        """The label capacity of the graph in `slot` (`initial` before the first capture), doubled until the batch's
+        labels fit.  It goes into the capture key, so only a batch with more labels than the capacity re-captures."""
+        cap = initial if getattr(self, slot) is None else getattr(self, slot)["cap"]
+        while cap < targets.shape[0]:
+            cap *= 2
+        return cap
+
+    def _static_labels(self, g, cap, targets):
+        """g["targets"] [cap, 6] fp32 and g["nt"] int32[1], filled from the capturing call.  The loss (ComputeLoss(...,
+        n_dev)) and LabelMatch's histogram read only the first nt rows, so one graph serves every label count <= cap."""
+        nt = int(targets.shape[0])
+        g.update(cap=cap, targets=torch.zeros((cap, 6), dtype=torch.float32, device=self.device),
+                 nt=torch.full((1,), nt, dtype=torch.int32, device=self.device))
+        g["targets"][:nt].copy_(targets)
+
+    def _stage_labels(self, g, targets):
+        """one call's labels (CPU or CUDA) into the static buffers, stream-ordered, without a host sync"""
+        nt = int(targets.shape[0])
+        g["targets"][:nt].copy_(targets, non_blocking=True)
+        # pageable source: the runtime stages these few bytes before returning, so the next step cannot overwrite them early
+        g["nt"].copy_(torch.tensor([nt], dtype=torch.int32))
 
     # ---- the whole step as CUDA graphs ------------------------------------------------------------------------------
     def _graphed(self, slot, key, hooks, inputs, ni):
@@ -346,7 +373,10 @@ class SSODTrainerStep(TrainerStep):
 
     # trainer/ssod_trainer.py:587-680 (logging / meters excluded: rank-0 host bookkeeping)
     def train_instance(self, imgs, targets, unlabeled_imgs, unlabeled_imgs_ori, unlabeled_gt, unlabeled_M, ni,
-                       host_pseudo_labels=False, _stop_after_backward=False):
+                       host_pseudo_labels=False, _stop_after_backward=False, _n_dev=None):
+        """_stop_after_backward: the body of the captured graph A (TrainerStep._graphed), which ends after the backward and
+        leaves LabelMatch's image counters to the replay wrapper.  _n_dev (int32[1] CUDA): targets is a padded label
+        buffer whose first _n_dev rows are the labels (ComputeLoss(..., n_dev), LabelMatch.update_device(..., n_dev))."""
         self._require_semi_ema()
         n_img = imgs.shape[0]
         self._mark("start")
@@ -369,9 +399,9 @@ class SSODTrainerStep(TrainerStep):
                 (teacher_pred, train_out), teacher_feature = self.ema.ema(unlabeled_imgs_ori, augment=False)
             self._mark("teacher_forward")
             if hasattr(self.pseudo_label_creator, "update_device"):      # LabelMatch: ssod_trainer.py:616-617 (labeled-target histogram)
-                self.pseudo_label_creator.update_device(targets)
-                self.pseudo_label_creator.count += imgs.shape[0]
-                self.pseudo_label_creator.pse_count += unlabeled_imgs.shape[0]
+                self.pseudo_label_creator.update_device(targets, _n_dev)
+                if not _stop_after_backward:
+                    self._count_labelmatch_images(imgs, unlabeled_imgs)
             if host_pseudo_labels:   # the reference's return contract: CPU float64 rows + flag (one D2H sync)
                 unlabeled_targets, invalid_target_shape = self.pseudo_label_creator.create_pseudo_label_online_with_gt(
                     teacher_pred, unlabeled_imgs, unlabeled_M, unlabeled_imgs_ori, unlabeled_gt, self.RANK)
@@ -393,7 +423,7 @@ class SSODTrainerStep(TrainerStep):
             total_pred, total_feature = self.model([imgs, unlabeled_imgs])
         self._mark("student_forward")
         sup_pred, sup_feature, un_sup_pred, un_sup_feature = self.split_predict_and_feature(total_pred, total_feature, n_img)
-        sup_loss, sup_loss_items = self.compute_loss(sup_pred, targets)
+        sup_loss, sup_loss_items = self.compute_loss(sup_pred, targets, _n_dev)
         d_loss = self.domain_loss(sup_feature)
         t_loss = self.target_loss(un_sup_feature)
         if self.cfg.SSOD.with_da_loss:
@@ -424,46 +454,62 @@ class SSODTrainerStep(TrainerStep):
 
     # ---- the whole step as CUDA graphs ------------------------------------------------------------------------------
     def _ssod_static(self, key, imgs, targets, us, uw, Ms):
-        return dict(imgs=imgs.clone(), targets=targets.clone(), us=us.clone(), uw=uw.clone(), Ms=Ms.to(self.device, torch.float64).clone())
+        g = dict(imgs=imgs.clone(), us=us.clone(), uw=uw.clone(), Ms=Ms.to(self.device, torch.float64).clone())
+        self._static_labels(g, key[-1], targets)
+        self.captures += 1
+        return g
 
     def _ssod_stage(self, g, imgs, targets, us, uw, Ms):
         g["imgs"].copy_(imgs, non_blocking=True)
-        g["targets"].copy_(targets, non_blocking=True)
+        self._stage_labels(g, targets)
         g["us"].copy_(us, non_blocking=True)
         g["uw"].copy_(uw, non_blocking=True)
         g["Ms"].copy_(Ms, non_blocking=True)
 
     def _ssod_body(self, g):
-        return self.train_instance(g["imgs"], g["targets"], g["us"], g["uw"], None, g["Ms"], None, _stop_after_backward=True)
+        return self.train_instance(g["imgs"], g["targets"], g["us"], g["uw"], None, g["Ms"], None, _stop_after_backward=True,
+                                   _n_dev=g["nt"])
 
     _SSOD_GRAPH = GraphHooks(_ssod_static, _ssod_stage, _ssod_body,
                              lambda self, scalars_dev: update_ema_pair(self.ema, self.semi_ema, self.model, scalars_dev=scalars_dev),
                              lambda self: next_pair_decays(self.ema, self.semi_ema))
 
     def train_instance_graphed(self, imgs, targets, unlabeled_imgs, unlabeled_imgs_ori, unlabeled_gt, unlabeled_M, ni):
-        """train_instance captured once (static shapes, device-resident pseudo labels, no host sync anywhere in the step)
+        """train_instance captured once per image shape (device-resident pseudo labels, no host sync anywhere in the step)
         and replayed as two graphs (TrainerStep._graphed): A = teacher forward ... backward, B = SGD-Nesterov + both EMA
-        updates."""
+        updates.  The labels go into a static buffer of capacity C with their count on the device (_static_labels), so
+        any label count up to C replays the same graph; a batch with more re-captures once, with C doubled until it fits."""
         self._require_semi_ema()
-        key = (tuple(imgs.shape), tuple(targets.shape), tuple(unlabeled_imgs.shape), tuple(unlabeled_M.shape),
-               imgs.dtype, unlabeled_imgs.dtype, unlabeled_imgs_ori.dtype)      # uint8 loader batches vs fp32: different static buffers
+        cap = self._label_capacity("_graph", targets, self.LABEL_CAPACITY)
+        key = (tuple(imgs.shape), tuple(unlabeled_imgs.shape), tuple(unlabeled_M.shape),
+               imgs.dtype, unlabeled_imgs.dtype, unlabeled_imgs_ori.dtype, cap)   # uint8 loader batches vs fp32: different static buffers
         loss = self._graphed("_graph", key, self._SSOD_GRAPH, (imgs, targets, unlabeled_imgs, unlabeled_imgs_ori, unlabeled_M), ni)
-        if hasattr(self.pseudo_label_creator, "stage_detections"):   # LabelMatch: the captured step cannot stage its detections itself
+        if hasattr(self.pseudo_label_creator, "stage_detections"):   # LabelMatch: the captured body neither stages nor counts
             self.pseudo_label_creator.stage_detections()
+            self._count_labelmatch_images(imgs, unlabeled_imgs)
         return loss
 
+    def _count_labelmatch_images(self, imgs, unlabeled_imgs):
+        """LabelMatch.update's image counters (labelmatch.py:126-129): host integers, advanced once per step"""
+        self.pseudo_label_creator.count += imgs.shape[0]
+        self.pseudo_label_creator.pse_count += unlabeled_imgs.shape[0]
+
     def _snapshot_training_state(self):
-        """+ the LabelMatch image counters, which the SSOD warm-up steps before a capture advance"""
+        """+ LabelMatch's state that the SSOD warm-up steps before a capture touch: the device class histogram, the staged
+        detections and the image counters"""
         restore = super()._snapshot_training_state()
         c = self.pseudo_label_creator
-        if not hasattr(c, "count"):
+        if not hasattr(c, "class_hist"):
             return restore
-        counts = (c.count, c.pse_count)
+        saved = (c.count, c.pse_count, list(c._pending))
+        hist = c.class_hist(self.device)
+        hist_snap = hist.clone()
 
-        def restore_with_counts():
+        def restore_labelmatch():
             restore()
-            c.count, c.pse_count = counts
-        return restore_with_counts
+            c.count, c.pse_count, c._pending = saved
+            hist.copy_(hist_snap)
+        return restore_labelmatch
 
     def after_epoch(self, epoch, start_epoch=0):
         """ssod_trainer.py:319-323: LabelMatch re-estimates the per-class thresholds once per epoch; the unsupervised loss
@@ -561,29 +607,21 @@ class SSODTrainerStep(TrainerStep):
         than C labels re-captures with C doubled until it fits."""
         if self.semi_ema is not None:
             raise RuntimeError("burn-in step requested after the hand-over to the semi-supervised phase (semi_ema exists)")
-        cap = self.BURN_IN_LABEL_CAPACITY if self._burn_graph is None else self._burn_graph["cap"]
-        while cap < targets.shape[0]:
-            cap *= 2
+        cap = self._label_capacity("_burn_graph", targets, self.BURN_IN_LABEL_CAPACITY)
         key = (tuple(imgs.shape), imgs.dtype, None if uw is None else (tuple(uw.shape), uw.dtype), cap)
         return self._graphed("_burn_graph", key, self._BURN_IN_GRAPH, (imgs, targets, uw), ni)
 
     def _burn_in_static(self, key, imgs, targets, uw):
-        cap, nt = key[-1], int(targets.shape[0])
-        g = dict(cap=cap, imgs=imgs.clone(), uw=None if uw is None else uw.clone(),
-                 targets=torch.zeros((cap, 6), dtype=torch.float32, device=self.device),
-                 nt=torch.full((1,), nt, dtype=torch.int32, device=self.device))
-        g["targets"][:nt].copy_(targets)
+        g = dict(imgs=imgs.clone(), uw=None if uw is None else uw.clone())
+        self._static_labels(g, key[-1], targets)
         self.burn_in_captures += 1
         return g
 
     def _burn_in_stage(self, g, imgs, targets, uw):
-        nt = int(targets.shape[0])
         g["imgs"].copy_(imgs, non_blocking=True)
         if uw is not None:
             g["uw"].copy_(uw, non_blocking=True)
-        g["targets"][:nt].copy_(targets, non_blocking=True)
-        # pageable source: the runtime stages these few bytes before returning, so the next step cannot overwrite them early
-        g["nt"].copy_(torch.tensor([nt], dtype=torch.int32))
+        self._stage_labels(g, targets)
 
     def _burn_in_forward_backward(self, g):
         # returns the loss detached: nothing may keep this step's autograd graph alive, because the AccumulateGrad nodes of
@@ -607,12 +645,12 @@ class SupTrainerStep(TrainerStep):
                  start_epoch=0):
         super().__init__(cfg, SupModel(cfg), device, rank, world_size, epochs, batch_size, amp_dtype, nb, start_epoch)
 
-    def _loss(self, imgs, targets):
+    def _loss(self, imgs, targets, n_dev=None):
         if self.WORLD_SIZE > 1 and not torch.cuda.is_current_stream_capturing():
             self._bn_broadcast()      # DDP broadcast_buffers=True (captured steps: _graphed issues it before the replay)
         with torch.autocast("cuda", dtype=self.amp_dtype):
             pred = self.model(imgs)
-        loss, _ = self.compute_loss(pred, targets)
+        loss, _ = self.compute_loss(pred, targets, n_dev)
         return loss
 
     def train_step(self, imgs, targets, ni):
@@ -621,23 +659,29 @@ class SupTrainerStep(TrainerStep):
         return loss.detach()
 
     def _static(self, key, imgs, targets):
-        return dict(imgs=imgs.clone(), targets=targets.clone())
+        g = dict(imgs=imgs.clone())
+        self._static_labels(g, key[-1], targets)
+        self.captures += 1
+        return g
 
     def _stage(self, g, imgs, targets):
         g["imgs"].copy_(imgs, non_blocking=True)
-        g["targets"].copy_(targets, non_blocking=True)
+        self._stage_labels(g, targets)
 
     def _forward_backward(self, g):
-        loss = self._loss(g["imgs"], g["targets"])
+        loss = self._loss(g["imgs"], g["targets"], g["nt"])
         self._backward(loss)
         return loss.detach()
 
     _GRAPH = GraphHooks(_static, _stage, _forward_backward, TrainerStep._ema_update_dev, TrainerStep._ema_decays)
 
     def train_step_graphed(self, imgs, targets, ni):
-        """train_step replayed from two captured CUDA graphs (TrainerStep._graphed, static shapes): A = forward + loss +
-        backward, B = SGD-Nesterov + the ModelEMA update with its decay read from device memory."""
-        key = (tuple(imgs.shape), tuple(targets.shape), imgs.dtype)
+        """train_step replayed from two captured CUDA graphs (TrainerStep._graphed), captured once per image shape and
+        dtype: A = forward + loss + backward, B = SGD-Nesterov + the ModelEMA update with its decay read from device
+        memory.  The labels go into a static buffer of capacity C with their count on the device (_static_labels); a
+        batch with more than C labels re-captures once, with C doubled until it fits."""
+        cap = self._label_capacity("_graph", targets, self.LABEL_CAPACITY)
+        key = (tuple(imgs.shape), imgs.dtype, cap)
         return self._graphed("_graph", key, self._GRAPH, (imgs, targets), ni)
 
 
@@ -647,25 +691,35 @@ class DevicePrefetcher:
     trainer/ssod_trainer.py:694-696).  put(batch of pinned host tensors) enqueues the copies into the next slot;
     get() makes the current stream wait for the oldest slot and returns its device tensors.  A slot is reused two put()s
     later, i.e. after the step that consumed it has been enqueued on the compute stream -- put() makes the copy stream wait
-    for that point before overwriting."""
+    for that point before overwriting.  A tensor whose first dimension changes between batches (the labels: a different
+    count almost every batch) gets a slot buffer that grows by doubling, and get() returns a view of the batch's length."""
 
     def __init__(self, device, slots=2):
         self.device = torch.device(device)
         self.stream = torch.cuda.Stream(self.device)
-        self.slots = [dict(buf=None, ready=torch.cuda.Event(), free=None) for _ in range(slots)]
+        self.slots = [dict(buf={}, view={}, ready=torch.cuda.Event(), free=None) for _ in range(slots)]
         self.head = self.tail = 0          # next slot to fill / next slot to hand out
         self.pending = 0
 
     def put(self, batch):
         assert self.pending < len(self.slots), "prefetcher full: call get() first"
         sl = self.slots[self.head]
-        if sl["buf"] is None:
-            sl["buf"] = {k: torch.empty(v.shape, dtype=v.dtype, device=self.device) for k, v in batch.items()}
         if sl["free"] is not None:
             self.stream.wait_event(sl["free"])          # the consumer of this slot's previous contents has been enqueued and finished
         with torch.cuda.stream(self.stream):
             for k, v in batch.items():
-                sl["buf"][k].copy_(v, non_blocking=True)
+                buf = sl["buf"].get(k)
+                if buf is None or buf.dtype != v.dtype or buf.shape[1:] != v.shape[1:] or buf.shape[0] < v.shape[0]:
+                    n = v.shape[0]
+                    if buf is not None and buf.dtype == v.dtype and buf.shape[1:] == v.shape[1:]:
+                        n = max(buf.shape[0], 1)
+                        while n < v.shape[0]:
+                            n *= 2
+                    # allocated on the copy stream after its wait on `free`: the old buffer goes back to this stream's pool
+                    # only once the compute stream has finished reading it
+                    buf = sl["buf"][k] = torch.empty((n,) + tuple(v.shape[1:]), dtype=v.dtype, device=self.device)
+                view = sl["view"][k] = buf[:v.shape[0]]
+                view.copy_(v, non_blocking=True)
             sl["ready"].record(self.stream)
         self.head = (self.head + 1) % len(self.slots)
         self.pending += 1
@@ -678,7 +732,7 @@ class DevicePrefetcher:
         self._last = sl
         self.tail = (self.tail + 1) % len(self.slots)
         self.pending -= 1
-        return sl["buf"]
+        return dict(sl["view"])
 
     def release(self):
         """call after the kernels that read the last get()'s tensors have been enqueued on the current stream"""

@@ -166,6 +166,16 @@ int etb_build_targets(const float* targets, const int32_t* nt_dev, int32_t nt_ho
                       const EtbAssignLevels* lv, const EtbAssignOut* out, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * LabelMatch.update's class histogram of the labeled rows, `cls_tmp[int(l[1:2])] += 1`
+ * (utils/labelmatch.py:126-134).  targets [cap,tstride] fp32, class in column 1; the row count is *n_dev if
+ * n_dev is non-NULL, else n_host (<= cap); rows past it are never read.  ADDS into hist[nc+1] int32: class =
+ * the float truncated toward zero; a class outside [0,nc) (or NaN) is counted in hist[nc].  No host sync, no
+ * allocation, order-independent (integer atomics): capturable in a CUDA graph.
+ * ------------------------------------------------------------------------------------------- */
+int etb_label_class_hist(const float* targets, const int32_t* n_dev, int32_t n_host, int32_t cap, int32_t tstride,
+                         int32_t nc, int32_t* hist, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * bbox_iou, CIoU branch, xywh 1-to-1 (utils/metrics.py:207-249).  box1,box2 [n,4] fp32 -> out [n].
  * ------------------------------------------------------------------------------------------- */
 int etb_bbox_ciou(const float* box1, const float* box2, int32_t n, float* out, void* stream);
