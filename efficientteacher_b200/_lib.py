@@ -152,6 +152,12 @@ _SIGS = {
     "etb_domain_focal_bwd": (C.c_int, [C.POINTER(EtbFocalParams), vp, vp]),
     "etb_val_process_batch": (C.c_int, [vp, vp, C.c_int32, C.c_int32, C.c_int32, vp, C.c_int32, vp, C.c_int32, vp, vp, vp]),
     "etb_nms_boxes": (C.c_int, [vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_float, vp, vp, vp]),
+    "etb_val_epoch_append_workspace_bytes": (C.c_size_t, [C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
+    "etb_val_epoch_append": (C.c_int, [vp, vp, C.c_int32, C.c_int32, C.c_int32, vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                       vp, C.c_int32, C.c_int32, vp, vp, vp, C.c_int64, vp, vp, vp, vp, C.c_size_t, vp]),
+    "etb_ap_per_class_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int32]),
+    "etb_ap_per_class": (C.c_int, [vp, vp, vp, C.c_int64, C.c_int32, vp, C.c_int32, C.c_int32, vp, vp, vp, vp, vp, vp, vp, vp,
+                                   C.c_size_t, vp]),
     "etb_stem_im2col_into": (C.c_int, [vp, C.c_int32, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_float, vp]),
     "etb_tal_workspace_bytes": (C.c_size_t, [C.c_int32, C.c_int32, C.c_int32]),
     "etb_tal_assign": (C.c_int, [vp, vp, vp, vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_float, C.c_float,

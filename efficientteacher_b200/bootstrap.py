@@ -15,9 +15,11 @@ trainer/ssod_trainer.py:261) on the original class.  apply() does three things:
 Modules of the host application imported later with `from X import Y` see the patched attribute of X anyway.
 """
 import importlib
+import inspect
 import sys
 
-from . import _lib, ema, labelmatch, loss, model, nms, pseudo_label, ssod_loss, assigner, tal
+from . import _lib, ema, labelmatch, loss, metrics, model, nms, pseudo_label, ssod_loss, assigner, tal
+from . import val as etb_val
 
 _lib.lib()  # fail loudly now if the kernels are not built
 
@@ -47,6 +49,35 @@ def _bbox_iou(original):
     return bbox_iou
 
 
+def _val_run(original):
+    """val.run (val.py:149-465): the training-time call (model and dataloader given, CUDA, plots=False, no txt / json /
+    hybrid output, no keypoints, no model_post, no augment) runs natively (efficientteacher_b200.val.run); every other call
+    goes to the host application's own run."""
+    sig = inspect.signature(etb_val.run)
+
+    def run(*args, **kwargs):
+        try:
+            bound = sig.bind(*args, **kwargs)
+        except TypeError:
+            return run.__wrapped__(*args, **kwargs)
+        if etb_val.run_unsupported(**bound.arguments) is None:
+            return etb_val.run(*args, **kwargs)
+        return run.__wrapped__(*args, **kwargs)
+    run.__wrapped__ = original
+    return run
+
+
+def _ap_per_class(original):
+    """utils.metrics.ap_per_class (metrics.py:22-126): native (efficientteacher_b200.metrics); plot=True (the PR / F1 plots)
+    goes to the host application's own function."""
+    def ap_per_class(tp, conf, pred_cls, target_cls, plot=False, save_dir='.', names=()):
+        if plot:
+            return ap_per_class.__wrapped__(tp, conf, pred_cls, target_cls, plot=plot, save_dir=save_dir, names=names)
+        return metrics.ap_per_class(tp, conf, pred_cls, target_cls)
+    ap_per_class.__wrapped__ = original
+    return ap_per_class
+
+
 # (defining module, attribute, replacement | factory(original) -> replacement)
 _PATCHES = [
     ("utils.torch_utils", "ModelEMA", ema.ModelEMA),
@@ -55,6 +86,8 @@ _PATCHES = [
     ("utils.general", "non_max_suppression_ssod", nms.non_max_suppression_ssod),
     ("utils.general", "non_max_suppression", _val_nms),
     ("utils.metrics", "bbox_iou", _bbox_iou),
+    ("utils.metrics", "ap_per_class", _ap_per_class),
+    ("val", "run", _val_run),
     ("utils.self_supervised_utils", "FairPseudoLabel", pseudo_label.FairPseudoLabel),
     ("utils.labelmatch", "LabelMatch", labelmatch.LabelMatch),
     ("models.loss.loss", "ComputeLoss", loss.ComputeLoss),
@@ -64,7 +97,10 @@ _PATCHES = [
     ("models.detector.yolo_ssod", "Model", model.Model),
     ("models.detector.yolo", "Model", model.SupModel),
 ]
-_FACTORIES = (_val_nms, _bbox_iou)
+_FACTORIES = (_val_nms, _bbox_iou, _ap_per_class, _val_run)
+# defining modules whose import may fail (val.py pulls in optional dependencies of the host application): their patches are
+# skipped, listed in apply.skipped
+_OPTIONAL = ("val",)
 # modules of the host application that bind the names above with `from X import Y` (imported here when possible so that the
 # sweep reaches them; a missing optional dependency of one of them only skips that module)
 _BINDERS = ["models.loss", "loss.loss", "models.assigner", "models.backbone.common", "trainer.trainer", "trainer.ssod_trainer", "val"]
@@ -78,21 +114,28 @@ def _is_original(obj, attr, mod_name):
 
 def apply(import_binders=True):
     """Returns the sorted list of `module.attribute` names that were rebound."""
-    for mod_name, _, _ in _PATCHES:
+    skipped = []
+    for mod_name in dict.fromkeys(m for m, _, _ in _PATCHES):
         try:
             importlib.import_module(mod_name)
         except Exception as e:  # the host application is not on sys.path
+            if mod_name in _OPTIONAL:
+                skipped.append((mod_name, repr(e)))
+                continue
             raise RuntimeError("efficientteacher_b200.bootstrap: cannot import reference module %s (%s)" % (mod_name, e))
-    skipped = []
     if import_binders:
         for mod_name in _BINDERS:
+            if mod_name in sys.modules or any(mod_name == m for m, _ in skipped):
+                continue
             try:
                 importlib.import_module(mod_name)
             except Exception as e:
                 skipped.append((mod_name, repr(e)))
     done = []
     for mod_name, attr, repl in _PATCHES:
-        defining = sys.modules[mod_name]
+        defining = sys.modules.get(mod_name)
+        if defining is None:     # an optional module that could not be imported
+            continue
         originals = {}
         for m in list(sys.modules.values()):
             d = getattr(m, "__dict__", None)

@@ -15,7 +15,9 @@ MAX_WH = 7680.0   # general.py:910 / :1013
 MAX_NMS = 30000   # general.py:911 / :1014
 
 
-def _run(prediction, conf_thres, iou_thres, agnostic, max_det, need_cls_conf, Ms=None, img_hw=(0, 0)):
+def _run(prediction, conf_thres, iou_thres, agnostic, max_det, need_cls_conf, Ms=None, img_hw=(0, 0), ws_name="nms"):
+    """ws_name: the cached workspace to use.  A captured training step bakes the pointer of "nms" into its graph, so a
+    caller with other batch shapes (validation) passes its own name: growing "nms" would free the captured buffer."""
     assert 0 <= conf_thres <= 1, f'Invalid Confidence threshold {conf_thres}, valid values are between 0.0 and 1.0'
     assert 0 <= iou_thres <= 1, f'Invalid IoU {iou_thres}, valid values are between 0.0 and 1.0'
     _lib.require_cuda(prediction)
@@ -34,7 +36,7 @@ def _run(prediction, conf_thres, iou_thres, agnostic, max_det, need_cls_conf, Ms
     p.img_h, p.img_w = int(img_hw[0]), int(img_hw[1])
     lib = _lib.lib()
     dev = pred.device
-    ws = _ws.workspace("nms", lib.etb_nms_workspace_bytes(C.byref(p)), dev)
+    ws = _ws.workspace(ws_name, lib.etb_nms_workspace_bytes(C.byref(p)), dev)
     det = torch.empty((B, max_det, 8), dtype=torch.float32, device=dev)
     det_cnt = torch.empty((B,), dtype=torch.int32, device=dev)
     pl_rows = pl_cnt = None

@@ -394,6 +394,36 @@ int etb_val_process_batch(const float* det, const int32_t* det_cnt, int32_t B, i
                           const float* labels, int32_t nt, const float* iouv, int32_t T, uint8_t* correct,
                           int32_t* overflow_dev, void* stream);
 
+/* one validation batch into the epoch's statistics (val.py:340-376), no host sync: det [B][max_det][det_ld>=6] etb_nms_val rows
+ * (x1,y1,x2,y2,conf,cls in the letterboxed H x W image), det_cnt [B]; img_meta [B][5] fp32 (h0, w0, inv_gain, padw, padh
+ * from the loader's shapes[b] = ((h0, w0), ((gain, _), (padw, padh))), inv_gain = fp32(1 / gain) with the division in
+ * float64); targets [nt][6] fp32 (img, cls, x, y, w, h normalised).  Rows are rescaled to native space as torch does it on
+ * fp32 CUDA tensors (x - pad, times inv_gain -- torch divides by a host scalar that way --, clamp to the native image),
+ * class 0 if single_cls; labels become native xyxy; etb_val_process_batch matches them (iouv [T], T <= 16).  Each detection's conf, class and correct bits (bit i = IoU threshold i) are appended to arena_conf / arena_cls /
+ * arena_tp at rows [*arena_n, ...) and *arena_n advances; label classes are ADDED into hist[nc+1] (etb_label_class_hist).
+ * flags[0] |= 1 if any appended bit is set; flags[1] = 1 on overflow (an image with more than 1024 labels, or rows past
+ * arena_cap, which are dropped).  workspace: etb_val_epoch_append_workspace_bytes(B, max_det, nt, T). */
+size_t etb_val_epoch_append_workspace_bytes(int32_t B, int32_t max_det, int32_t nt, int32_t T);
+int etb_val_epoch_append(const float* det, const int32_t* det_cnt, int32_t B, int32_t max_det, int32_t det_ld,
+                         const float* img_meta, const float* targets, int32_t nt, int32_t H, int32_t W, int32_t single_cls,
+                         const float* iouv, int32_t T, int32_t nc, float* arena_conf, float* arena_cls, uint16_t* arena_tp,
+                         int64_t arena_cap, int64_t* arena_n, int32_t* hist, int32_t* flags, void* workspace,
+                         size_t workspace_bytes, void* stream);
+
+/* numeric core of ap_per_class (utils/metrics.py:22-126) over n rows conf [n] fp32, pred_cls [n] fp32, tp [n] uint16 (bit t =
+ * true positive at IoU column t, T <= 16).  cls_slot [ncls_table]: the slot (0..nu-1, in ascending class order) of every
+ * class that has labels, -1 otherwise; a row whose class is not an integer in [0, ncls_table) with a slot is ignored.
+ * n_l [nu] labels per slot.  Rows are sorted by (slot, conf descending) with a stable radix sort (equal confidences keep their
+ * row order).  px [1000] = numpy.linspace(0, 1, 1000), xs [101] = numpy.linspace(0, 1, 101).  Outputs (float64):
+ * ap_points [nu][T][101] = numpy.interp(xs, mrec, envelope(mpre)) of compute_ap, p_curve / r_curve [nu][1000] = the P and R
+ * curves at column 0 (numpy.interp(-px, -conf, ., left=1 / 0)), zero for a slot without predictions; n_p [nu] int32.
+ * Recall must not decrease along a class (at most n_l true positives per column).
+ * workspace: etb_ap_per_class_workspace_bytes(n, nu). */
+size_t etb_ap_per_class_workspace_bytes(int64_t n, int32_t nu);
+int etb_ap_per_class(const float* conf, const float* pred_cls, const uint16_t* tp, int64_t n, int32_t T, const int32_t* cls_slot,
+                     int32_t ncls_table, int32_t nu, const int32_t* n_l, const double* px, const double* xs, double* ap_points,
+                     double* p_curve, double* r_curve, int32_t* n_p, void* workspace, size_t workspace_bytes, void* stream);
+
 /* class-agnostic greedy NMS over ready-made detection rows (extra-teachers merge, utils/self_supervised_utils.py:256-274,
  * torchvision.ops.nms semantics): rows [B][nmax<=1024][ld>=5] fp32 (x1,y1,x2,y2,score,...), cnt [B]; kept rows are written
  * to out [B][nmax][ld] in descending-score (stable) order, out_cnt [B]. */
