@@ -15,7 +15,8 @@
 //   * warpgroup roles: warpgroup 0 is the TMA producer (one elected lane of its first warp issues), warpgroups 1 and 2
 //     each own 64 of the 128 pixel rows and issue wgmma.m64nBNk16 x4 per stage; the fp32 accumulator lives in their
 //     registers, and the epilogue (folded BN scale/bias -> SiLU -> +residual -> bf16 NHWC store at a channel offset of a
-//     wider buffer, so torch.cat is free) runs straight from those registers.
+//     wider buffer, so torch.cat is free) runs straight from those registers; the raw-output epilogue (EPI 0) stages the
+//     tile through shared memory first and stores whole pixel rows.
 //   * every mbarrier wait is bounded (trap after ~2 s) so a descriptor bug cannot hang the GPU.
 #include "common.cuh"
 #include <cuda.h>
@@ -173,14 +174,19 @@ struct ConvKArgs {
   float* y_f32;
 };
 
-template <int BN>
+// EPI 0 stages each consumer warpgroup's fp32 accumulator through shared memory, half of its columns at a time
+// (64 rows x BN/2 fp32: 16 KB at BN = 128), so the global store goes out in 16 B vectors along the pixel rows.
+template <int BN, int EPI>
 struct ConvSmem {
   static constexpr int A_BYTES = CONV_BLOCK_M * 128;
   static constexpr int B_BYTES = BN * 128;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int STAGES = CONV_SMEM_STAGES_BYTES / STAGE_BYTES;   // 6 (BN = 128) or 8 (BN = 64)
-  static constexpr int BAR_OFF = STAGES * STAGE_BYTES;
+  static constexpr int OUT_BYTES = EPI == 0 ? 64 * (BN / 2) * 4 : 0;   // per consumer warpgroup
+  static constexpr int OUT_OFF = STAGES * STAGE_BYTES;
+  static constexpr int BAR_OFF = OUT_OFF + 2 * OUT_BYTES;
   static constexpr int TOTAL = BAR_OFF + 256 + 1024;        // + barriers + slack for the 1024 B alignment
+  static_assert(TOTAL <= 227 * 1024, "shared memory per block");
 };
 
 __device__ __forceinline__ float conv_act(float x, int act) {
@@ -191,8 +197,8 @@ __device__ __forceinline__ float conv_act(float x, int act) {
 
 // Epilogue of one consumer warpgroup's 64 x BN accumulator, straight from the wgmma fragment (see wgmma_m64n*k16): this
 // thread owns pixel rows r0 and r0+8 and, per 8-column block j, the channel pair 8j + 2*(lane%4) + {0,1}.  EPI selects the
-// fused tail at compile time so every register array is statically indexed:
-//   EPI 0: raw bf16 store (+= existing when a.accumulate)       -- dgrad, training forward
+// fused tail at compile time so every register array is statically indexed (EPI 0 is conv_epilogue_staged below):
+//   EPI 0: raw bf16 store (+= existing when a.accumulate)       -- dgrad, training forward (conv_epilogue_staged)
 //   EPI 1: v*scale+bias (folded BN) -> SiLU/ReLU -> (+residual) -- teacher forward
 //   EPI 2: +bias, fp32 scatter into the Detect layout           -- head
 //   EPI 3: EPI 1 with Hardswish                                 -- teacher forward of Hardswish layers
@@ -234,18 +240,101 @@ __device__ __forceinline__ void conv_epilogue(const ConvKArgs& a, const float* d
           v1 += rf.y;
         }
       }
-      if (pair) {
-        if (EPI == 0 && a.accumulate) {
-          const float2 pf = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(yp));
-          v0 += pf.x;
-          v1 += pf.y;
-        }
-        *reinterpret_cast<__nv_bfloat162*>(yp) = __floats2bfloat162_rn(v0, v1);
-      } else {
-        if (EPI == 0 && a.accumulate) v0 += __bfloat162float(*yp);
-        *yp = __float2bfloat16(v0);
+      if (pair) *reinterpret_cast<__nv_bfloat162*>(yp) = __floats2bfloat162_rn(v0, v1);
+      else *yp = __float2bfloat16(v0);
+    }
+  }
+}
+
+// Output pixel of row `row` (0..127) of a tile; false for rows outside the tile or the image.
+__device__ __forceinline__ bool conv_out_pixel(const ConvKArgs& a, int img, int th_i, int tw_i, int row, size_t* pix) {
+  const int th = row / a.TW, tw = row - th * a.TW;
+  const int oh = th_i * a.TH + th, ow = tw_i * a.TW + tw;
+  *pix = ((size_t)img * a.out_H + (size_t)(oh * a.out_os + a.out_ph)) * a.out_W + (size_t)(ow * a.out_os + a.out_pw);
+  return (row < a.TW * a.TH) && (oh < a.Ho) && (ow < a.Wo);
+}
+
+__device__ __forceinline__ void bar_sync_named(int id, int nthreads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
+__device__ __forceinline__ void st_shared_f2(uint32_t addr, float x, float y) {
+  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(x), "f"(y) : "memory");
+}
+__device__ __forceinline__ float4 ld_shared_f4(uint32_t addr) {
+  float4 v;
+  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr) : "memory");
+  return v;
+}
+
+// EPI 0: the warpgroup's 64 x BN accumulator goes out through its staging area `stg` (64 rows x BN/2 fp32) in two column
+// halves.  Each half: fragment -> stg (8 B stores), named barrier, then every thread takes 8 consecutive channels of one
+// row (two 16 B loads), adds the existing output when a.accumulate, rounds once to bf16 and stores 16 B, so a warp writes
+// whole 128-256 B runs of pixel rows instead of 8 rows x 16 B.  The values are those of a direct store from the fragment.
+// stg rows are 16 B chunks; chunk q of row r sits at q ^ 2*(r%4): the fragment stores (4 rows x 4 lanes per half-warp)
+// and the read-back (8 lanes of one 16 B phase take chunks 2g + h, h = bit 2 of the lane) are both free of bank conflicts.
+template <int BN>
+__device__ __forceinline__ void conv_epilogue_staged(const ConvKArgs& a, const float* d, int n0, int img, int th_i, int tw_i, int cw,
+                                                     uint32_t stg) {
+  constexpr int HALF = BN / 2;               // columns per half
+  constexpr int PITCH = HALF * 4;            // bytes per staged row
+  constexpr int GPR = HALF / 8;              // 8-channel groups per row: 8 (BN = 128) or 4 (BN = 64)
+  constexpr int RPI = 128 / GPR;             // rows read back per pass of the warpgroup
+  const int t = threadIdx.x & 127, lane = threadIdx.x & 31;
+  const int r_frag = 16 * (t >> 5) + (lane >> 2);
+  const int g = t % GPR, h = (lane >> 2) & 1;
+#pragma unroll
+  for (int hf = 0; hf < 2; ++hf) {
+    if (n0 + hf * HALF >= a.Cout) break;     // uniform: the whole half lies beyond Cout
+#pragma unroll
+    for (int jj = 0; jj < HALF / 8; ++jj) {
+      const int j = hf * (HALF / 8) + jj;
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const int r = r_frag + 8 * i;
+        const int q = 2 * jj + ((lane & 3) >> 1);
+        st_shared_f2(stg + r * PITCH + ((q ^ ((r & 3) << 1)) << 4) + ((lane & 1) << 3), d[j * 4 + i * 2], d[j * 4 + i * 2 + 1]);
       }
     }
+    bar_sync_named(1 + cw, 128);
+    const int gc = n0 + hf * HALF + 8 * g;
+#pragma unroll 1
+    for (int it = 0; it < 64 / RPI; ++it) {
+      const int r = it * RPI + t / GPR;
+      const int sw = (r & 3) << 1;
+      const float4 c0 = ld_shared_f4(stg + r * PITCH + (((2 * g + h) ^ sw) << 4));
+      const float4 c1 = ld_shared_f4(stg + r * PITCH + (((2 * g + 1 - h) ^ sw) << 4));
+      const float4 lo = h ? c1 : c0, hi = h ? c0 : c1;
+      float v[8] = {lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w};
+      size_t pix;
+      if (!conv_out_pixel(a, img, th_i, tw_i, 64 * cw + r, &pix) || gc >= a.Cout) continue;
+      __nv_bfloat16* yp = a.y + pix * a.y_cstride + a.y_coffset + gc;
+      if (gc + 8 <= a.Cout) {
+        if (a.accumulate) {
+          const uint4 pv = *reinterpret_cast<const uint4*>(yp);
+          const __nv_bfloat162* p2 = reinterpret_cast<const __nv_bfloat162*>(&pv);
+#pragma unroll
+          for (int k = 0; k < 4; ++k) {
+            const float2 f = __bfloat1622float2(p2[k]);
+            v[2 * k] += f.x;
+            v[2 * k + 1] += f.y;
+          }
+        }
+        uint4 o;
+        __nv_bfloat162* o2 = reinterpret_cast<__nv_bfloat162*>(&o);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) o2[k] = __floats2bfloat162_rn(v[2 * k], v[2 * k + 1]);
+        *reinterpret_cast<uint4*>(yp) = o;
+      } else {                                 // Cout % 8 != 0: the last group of channels is partial
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {
+          if (gc + k >= a.Cout) break;
+          float x = v[k];
+          if (a.accumulate) x += __bfloat162float(yp[k]);
+          yp[k] = __float2bfloat16(x);
+        }
+      }
+    }
+    bar_sync_named(1 + cw, 128);             // stg is rewritten by the next half / tile
   }
 }
 
@@ -255,7 +344,7 @@ __device__ __forceinline__ void conv_epilogue(const ConvKArgs& a, const float* d
 template <int BN, int EPI>
 __global__ void __launch_bounds__(CONV_THREADS, 1)
 conv_fwd_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB, const ConvKArgs a) {
-  using L = ConvSmem<BN>;
+  using L = ConvSmem<BN, EPI>;
   constexpr int STAGES = L::STAGES;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
@@ -340,17 +429,15 @@ conv_fwd_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
     const int tw_i = t % a.tiles_w; t /= a.tiles_w;
     const int th_i = t % a.tiles_h; t /= a.tiles_h;
     const int img = t;
-    bool row_ok[2];
-    size_t pix[2];
+    if constexpr (EPI == 0) {
+      conv_epilogue_staged<BN>(a, d, n0, img, th_i, tw_i, cw, smem_u32(smem + L::OUT_OFF + cw * L::OUT_BYTES));
+    } else {
+      bool row_ok[2];
+      size_t pix[2];
 #pragma unroll
-    for (int i = 0; i < 2; ++i) {
-      const int row = rbase + 8 * i;
-      const int th = row / a.TW, tw = row - th * a.TW;
-      const int oh = th_i * a.TH + th, ow = tw_i * a.TW + tw;
-      row_ok[i] = (row < a.TW * a.TH) && (oh < a.Ho) && (ow < a.Wo);
-      pix[i] = ((size_t)img * a.out_H + (size_t)(oh * a.out_os + a.out_ph)) * a.out_W + (size_t)(ow * a.out_os + a.out_pw);
+      for (int i = 0; i < 2; ++i) row_ok[i] = conv_out_pixel(a, img, th_i, tw_i, rbase + 8 * i, &pix[i]);
+      conv_epilogue<BN, EPI>(a, d, n0, row_ok, pix, lane);
     }
-    conv_epilogue<BN, EPI>(a, d, n0, row_ok, pix, lane);
   }
 }
 
@@ -386,7 +473,7 @@ static void pick_tile(int Wo, int Ho, int* TW, int* TH) {
 
 template <int BN, int EPI>
 static int launch_conv_e(const CUtensorMap& mA, const CUtensorMap& mB, const ConvKArgs& ka, dim3 grid, cudaStream_t st) {
-  using L = ConvSmem<BN>;
+  using L = ConvSmem<BN, EPI>;
   static bool attr_set = false;
   if (!attr_set) {
     ETB_CHECK_CUDA(cudaFuncSetAttribute(conv_fwd_kernel<BN, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::TOTAL));
