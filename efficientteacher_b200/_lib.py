@@ -29,6 +29,10 @@ class EtbSgdChunk(C.Structure):
     _fields_ = [("p", vp), ("g", vp), ("buf", vp), ("n", C.c_int32), ("group", C.c_int32)]
 
 
+class EtbAdamChunk(C.Structure):
+    _fields_ = [("p", vp), ("g", vp), ("m", vp), ("v", vp), ("n", C.c_int32), ("group", C.c_int32)]
+
+
 class EtbNmsParams(C.Structure):
     _fields_ = [("B", C.c_int32), ("P", C.c_int32), ("no", C.c_int32), ("conf_thres", C.c_float),
                 ("iou_thres", C.c_float), ("max_nms", C.c_int32), ("max_det", C.c_int32), ("max_wh", C.c_float),
@@ -93,6 +97,7 @@ _SIGS = {
     "etb_ema_update": (C.c_int, [vp, C.c_int64, C.c_float, C.c_float, C.c_float, C.c_float, vp]),
     "etb_ema_update_dev": (C.c_int, [vp, C.c_int64, vp, vp]),
     "etb_sgd_step": (C.c_int, [vp, C.c_int64, vp, C.c_int32, vp]),
+    "etb_adamw_step": (C.c_int, [vp, C.c_int64, vp, C.c_int32, vp]),
     "etb_detect_decode": (C.c_int, [vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                     C.c_int32, c_f32p, C.c_float, vp]),
     "etb_nms_workspace_bytes": (C.c_size_t, [C.POINTER(EtbNmsParams)]),

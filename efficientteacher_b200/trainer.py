@@ -26,7 +26,7 @@ from .domain_loss import DomainLoss, TargetLoss
 from .ema import ModelEMA, CosineEMA, SemiSupModelEMA, update_ema_pair, next_pair_decays, ema_scalars
 from .loss import ComputeLoss
 from .model import Model, SupModel
-from .optim import FusedSGD
+from .optim import FusedAdamW, FusedSGD
 from .parallel import GradArena
 from .pseudo_label import FairPseudoLabel
 from .ssod_loss import ComputeStudentMatchLoss
@@ -80,7 +80,7 @@ class TrainerStep:
         self._graph = None       # the step captured as CUDA graphs (see _graphed)
         self.captures = 0        # how many times _graph has been captured (train_instance_graphed / train_step_graphed)
 
-    # trainer/trainer.py:193-217
+    # trainer/trainer.py:193-247: FusedAdamW for `adam: True`, else FusedSGD, with the LambdaLR schedule
     def build_optimizer(self, cfg):
         nbs = 64
         self.accumulate = max(round(nbs / self.batch_size), 1)
@@ -93,7 +93,11 @@ class TrainerStep:
                 g_bnw.append(v.weight)
             elif hasattr(v, 'weight') and isinstance(v.weight, nn.Parameter):
                 g_w.append(v.weight)
-        self.optimizer = FusedSGD(g_b, lr=cfg.hyp.lr0, momentum=cfg.hyp.momentum, nesterov=True)   # one launch, zeroes the grads
+        if cfg.adam:
+            # groups 0 and 2 keep AdamW's default weight_decay (0.01), as torch fills it in for the reference
+            self.optimizer = FusedAdamW(g_b, lr=cfg.hyp.lr0, betas=(cfg.hyp.momentum, 0.999))      # one launch, zeroes the grads
+        else:
+            self.optimizer = FusedSGD(g_b, lr=cfg.hyp.lr0, momentum=cfg.hyp.momentum, nesterov=True)   # one launch, zeroes the grads
         self.optimizer.add_param_group({'params': g_w, 'weight_decay': weight_decay})
         self.optimizer.add_param_group({'params': g_bnw})
         if cfg.linear_lr:
@@ -101,6 +105,7 @@ class TrainerStep:
         else:
             self.lf = one_cycle(1, cfg.hyp.lrf, self.epochs)
         self.scheduler = torch.optim.lr_scheduler.LambdaLR(self.optimizer, lr_lambda=self.lf)
+        self.scheduler.last_epoch = self.epoch - 1     # trainer.py:247: the first scheduler.step() at an epoch's end gives lf(epoch)
         self.warmup_bias_lr, self.warmup_momentum, self.momentum = cfg.hyp.warmup_bias_lr, cfg.hyp.warmup_momentum, cfg.hyp.momentum
 
     # ---- gradient arena: all student gradients live in one flat fp32 buffer -> ONE all-reduce per step ----
@@ -250,7 +255,9 @@ class TrainerStep:
         if due:
             # pageable source: the runtime stages the 16 bytes before returning, so the next step cannot overwrite them early
             g["ema_dev"].copy_(torch.tensor(ema_scalars(*hooks.ema_decays(self)), dtype=torch.float32))
-            self.optimizer.refresh_hyper()   # lr / momentum of this step -> device memory read by the captured SGD kernel
+            # lr / momentum of this step -> device memory read by the captured SGD kernel (AdamW: the step count advances
+            # here, and this step's bias corrections go with the lr)
+            self.optimizer.refresh_hyper()
         self._bn_broadcast()
         g["graph"].replay()
         if due:
@@ -302,30 +309,36 @@ class TrainerStep:
 
     def _snapshot_training_state(self):
         """The warm-up steps before a capture really train: snapshot every piece of state they touch (weights, BN
-        statistics, the EMA model(s), momentum, the gradients accumulated towards the next optimizer step, the counters,
-        lr / momentum) and return the function that puts it back."""
+        statistics, the EMA model(s), the optimizer state -- SGD momentum, or AdamW's moments and step count --, the
+        gradients accumulated towards the next optimizer step, the counters, lr / momentum) and return the function that
+        puts it back."""
         self._ensure_arena()
         emas = [e for e in (self.ema, self.semi_ema) if e is not None]
+        opt_keys = ("momentum_buffer", "exp_avg", "exp_avg_sq")
         had_momentum = any(len(self.optimizer.state[p]) for g_ in self.optimizer.param_groups for p in g_["params"])
         tensors = [t for m in [self.model] + [e.ema for e in emas] for t in m.state_dict().values()]
         if had_momentum:
-            tensors += [self.optimizer.state[p]["momentum_buffer"] for g_ in self.optimizer.param_groups for p in g_["params"]
-                        if self.optimizer.state[p].get("momentum_buffer") is not None]
+            tensors += [self.optimizer.state[p][k] for g_ in self.optimizer.param_groups for p in g_["params"]
+                        for k in opt_keys if self.optimizer.state[p].get(k) is not None]
         tensors.append(self._arena.flat)     # gradients already accumulated towards the next optimizer step (accumulate > 1)
         snap = [t.clone() for t in tensors]
         saved = (self.last_opt_step, [e.updates for e in emas], self.accumulate,
                  [(x['lr'], x.get('momentum')) for x in self.optimizer.param_groups])
+        step_count = getattr(self.optimizer, "step_count", None)     # FusedAdamW's t of the bias corrections
 
         def restore():
             with torch.no_grad():
                 for t, c in zip(tensors, snap):
                     t.copy_(c)
-                if not had_momentum:      # buffers created by the warm-up: zero == "not yet created" for SGD (buf = grad on first use)
-                    for g_ in self.optimizer.param_groups:
+                if not had_momentum:      # state created by the warm-up: zero == "not yet created" (SGD: buf = grad on
+                    for g_ in self.optimizer.param_groups:    # first use; AdamW: zero moments with step_count 0)
                         for p in g_["params"]:
-                            b = self.optimizer.state[p].get("momentum_buffer")
-                            if b is not None:
-                                b.zero_()
+                            for k in opt_keys:
+                                b = self.optimizer.state[p].get(k)
+                                if b is not None:
+                                    b.zero_()
+            if step_count is not None:
+                self.optimizer.step_count = step_count
             self.last_opt_step, updates, self.accumulate, hyp = saved
             for e, u in zip(emas, updates):
                 e.updates = u
@@ -366,6 +379,14 @@ class SSODTrainerStep(TrainerStep):
         self._teacher_keep = None
         self._burn_graph = None     # captured burn-in step (train_without_unlabeled[_da]_graphed)
         self.burn_in_captures = 0   # how many times a burn-in step has been captured
+
+    # trainer/ssod_trainer.py:86-94: SSOD.multi_step_lr replaces the LambdaLR by MultiStepLR(milestones, gamma=0.1) on top
+    # of it (the warm-up still interpolates towards initial_lr * lf(epoch)); the supervised step has no such switch
+    def build_optimizer(self, cfg):
+        super().build_optimizer(cfg)
+        if cfg.SSOD.multi_step_lr:
+            self.scheduler = torch.optim.lr_scheduler.MultiStepLR(self.optimizer, milestones=cfg.SSOD.milestones, gamma=0.1)
+            self.scheduler.last_epoch = self.epoch - 1
 
     # "sum" = the reference (loss * WORLD_SIZE, then DDP's mean: trainer/ssod_trainer.py:638-648).  "avg" (ncclAvg: the same
     # collective at the same cost) is for synthetic benchmarks only: with SUM the effective learning rate grows with the world

@@ -84,6 +84,25 @@ typedef struct EtbSgdChunk {
 int etb_sgd_step(const EtbSgdChunk* table_dev, int64_t n_chunks, const float* hyper_dev, int32_t zero_grad, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Fused AdamW step over all parameters for `adam: True` (replaces torch.optim.AdamW.step + zero_grad; optimizer built in
+ * trainer/trainer.py:211-217: AdamW(g_b, lr=lr0, betas=(momentum, 0.999)) + conv-weight and BN-weight groups), the same
+ * arithmetic as torch's foreach AdamW (decoupled weight decay):
+ *   p *= 1-lr*wd ; m = lerp(m, g, 1-b1) ; v = v*b2 + (1-b2)*g*g ; p += (-lr/bc1) * m / (sqrt(v)/sqrt(bc2) + eps) ; (g = 0)
+ * chunk table like the SGD one (<= ETB_EMA_CHUNK elements per chunk); hyper_dev[8*group + 0..6] =
+ * {1-lr*wd, 1-b1, b2, 1-b2, -lr/bc1, sqrt(bc2), eps}, computed on the host in float64 and rounded once to fp32, in
+ * device memory so a captured CUDA graph follows the schedule and the bias corrections.
+ * ------------------------------------------------------------------------------------------- */
+typedef struct EtbAdamChunk {
+  float* p;
+  float* g;
+  float* m;       /* exp_avg    */
+  float* v;       /* exp_avg_sq */
+  int32_t n;
+  int32_t group;
+} EtbAdamChunk;
+int etb_adamw_step(const EtbAdamChunk* table_dev, int64_t n_chunks, const float* hyper_dev, int32_t zero_grad, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Detect eval-mode decode (models/head/yolov5_head.py:66-78): logits [B,na,ny,nx,no] of one level ->
  * rows of pred[B,P,no] at row offset `row0`:  sigmoid; xy=(2s-0.5+grid)*stride; wh=(2s)^2*anchor*stride.
  * ------------------------------------------------------------------------------------------- */
