@@ -12,28 +12,31 @@
 
 // ------------------------------------------------------------------------------------------------ Detect backward
 #define DET_PIX 64
-// grid (chunks, na, N), 128 threads: thread o < no walks DET_PIX pixels of (image n, anchor a): coalesced 340 B rows in,
-// 170 B runs out; per-channel partial sums of the bias gradient in registers -> partials[(n*chunks + chunk)][C].
+// grid (chunks, na, N), 128 threads: column j < no of (image n, anchor a) is channel a*no + j; the last anchor's block also
+// owns columns [no, no + Cpad - C), the pad channels [C, Cpad) (K padding of the dgrad GEMM), which it zeroes.  Thread t walks
+// the DET_PIX pixels of columns t, t + 128, ...: at no = 85 one column per thread, coalesced 340 B rows in, 170 B runs out;
+// per-channel partial sums of the bias gradient in registers -> partials[(n*chunks + chunk)][C].
 __global__ void __launch_bounds__(128) detect_dy_pack_kernel(const float* __restrict__ g, __nv_bfloat16* __restrict__ dy, float* __restrict__ partials,
                                                              int na, int HW, int no, int Cpad) {
   const int chunk = blockIdx.x, a = blockIdx.y, n = blockIdx.z;
-  const int o = threadIdx.x;
   const int C = na * no;
+  const int cols = a == na - 1 ? no + (Cpad - C) : no;
   const int p0 = chunk * DET_PIX, p1 = min(p0 + DET_PIX, HW);
   const float* gp = g + ((size_t)(n * na + a) * HW) * no;
   __nv_bfloat16* dp = dy + (size_t)n * HW * Cpad + a * no;
-  float acc = 0.f;
-  if (o < no) {
+  for (int o = threadIdx.x; o < cols; o += blockDim.x) {
+    if (o < no) {
+      float acc = 0.f;
 #pragma unroll 4
-    for (int p = p0; p < p1; ++p) {
-      const float v = __ldg(gp + (size_t)p * no + o);
-      acc += v;
-      dp[(size_t)p * Cpad + o] = __float2bfloat16(v);
+      for (int p = p0; p < p1; ++p) {
+        const float v = __ldg(gp + (size_t)p * no + o);
+        acc += v;
+        dp[(size_t)p * Cpad + o] = __float2bfloat16(v);
+      }
+      partials[((size_t)n * gridDim.x + chunk) * C + a * no + o] = acc;
+    } else {
+      for (int p = p0; p < p1; ++p) dp[(size_t)p * Cpad + o] = __float2bfloat16(0.f);
     }
-    partials[((size_t)n * gridDim.x + chunk) * C + a * no + o] = acc;
-  } else if (a == na - 1 && o - no < Cpad - C) {       // zero the pad channels [C, Cpad) (K padding of the dgrad GEMM)
-    __nv_bfloat16* zp = dy + (size_t)n * HW * Cpad + C + (o - no);
-    for (int p = p0; p < p1; ++p) zp[(size_t)p * Cpad] = __float2bfloat16(0.f);
   }
 }
 
@@ -58,8 +61,8 @@ extern "C" int64_t etb_detect_dy_rows(int32_t N, int32_t H, int32_t W) { return 
 
 extern "C" int etb_detect_dy_pack(const float* g, void* dy_bf16, float* partials, int32_t N, int32_t na, int32_t H, int32_t W, int32_t no,
                                   int32_t Cpad, void* stream) {
-  ETB_CHECK_ARG(g && dy_bf16 && partials && N > 0 && na > 0 && H > 0 && W > 0 && no > 0 && no <= 128);
-  ETB_CHECK_ARG(Cpad >= na * no && Cpad % 8 == 0 && no + (Cpad - na * no) <= 128 && na < 65536 && N < 65536);
+  ETB_CHECK_ARG(g && dy_bf16 && partials && N > 0 && na > 0 && H > 0 && W > 0 && no > 0);
+  ETB_CHECK_ARG(Cpad >= na * no && Cpad % 8 == 0 && na < 65536 && N < 65536);
   const int HW = H * W;
   dim3 grid((HW + DET_PIX - 1) / DET_PIX, na, N);
   etb_launch(detect_dy_pack_kernel, dim3(grid), dim3(128), 0, (cudaStream_t)stream, g, (__nv_bfloat16*)dy_bf16, partials, na, HW, no, Cpad);

@@ -374,7 +374,8 @@ int etb_pack_stem_weight(const float* w_oihw, void* w_bf16, int32_t Cout, void* 
  * models/head/yolov5_head.py:66).  etb_detect_dy_pack rewrites it as the bf16 NHWC operand dy [N,H,W,Cpad] (channel =
  * a*no + o, pad channels zeroed) of the wgmma dgrad / wgrad and emits per-block column sums; etb_column_sum reduces them
  * to the conv-bias gradient (yolov5_head.py:55: nn.Conv2d(..., bias=True)) -- replaces autograd's permute/contiguous/sum.
- * partials: [etb_detect_dy_rows(N,H,W)][na*no] floats. */
+ * Any no >= 1 and any Cpad >= na*no with Cpad % 8 == 0 (DetectConvFn passes ceil64(na*no)); every pad channel of dy is
+ * written (zero), so dy needs no initialisation.  partials: [etb_detect_dy_rows(N,H,W)][na*no] floats. */
 int64_t etb_detect_dy_rows(int32_t N, int32_t H, int32_t W);
 int etb_detect_dy_pack(const float* g, void* dy_bf16, float* partials, int32_t N, int32_t na, int32_t H, int32_t W,
                        int32_t no, int32_t Cpad, void* stream);

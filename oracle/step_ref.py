@@ -23,8 +23,13 @@ def domain_focal(feature, label):
 
 class CpuSSODStep:
     def __init__(self, state_dict, depth, neck_depth, lr=0.01, momentum=0.937, weight_decay=0.0005, batch_size=32,
-                 ema_updates=0, semi_decay=0.999, teacher_loss_weight=3.0, bn_momentum=0.0, warmup=None, fixed_accumulate=True):
-        """bn_momentum > 0: the student's running statistics are updated like nn.BatchNorm2d(momentum) does (needed for
+                 ema_updates=0, semi_decay=0.999, teacher_loss_weight=3.0, bn_momentum=0.0, warmup=None, fixed_accumulate=True,
+                 nc=80, anchor_t=4.0, da_loss_weight=0.0):
+        """nc / anchor_t: the dataset's class count and Loss.anchor_t; the class-loss weight is derived from nc as
+        ComputeLoss / ComputeStudentMatchLoss do (cls * nc / 80 * 3 / nl, models/loss/loss.py:124), and the per-class
+        pseudo-label thresholds are sized by it.  da_loss_weight: SSOD.da_loss_weights when SSOD.with_da_loss is on (the
+        domain losses of the labeled and unlabeled halves join the supervised loss, trainer/ssod_trainer.py:633-636), else 0.
+        bn_momentum > 0: the student's running statistics are updated like nn.BatchNorm2d(momentum) does (needed for
         multi-step trajectories; the single-step parity tests leave it 0).  warmup = (nw, warmup_bias_lr, warmup_momentum):
         apply the reference's per-iteration warm-up (trainer/trainer.py:388-395: group index 2 gets warmup_bias_lr)."""
         self.bn_momentum, self.warmup, self.lr0, self.momentum0, self.ni = bn_momentum, warmup, lr, momentum, 0
@@ -49,6 +54,8 @@ class CpuSSODStep:
         self.opt.add_param_group({'params': g_w, 'weight_decay': wd})
         self.opt.add_param_group({'params': g_bn})
         self.ema_updates, self.semi_decay, self.tlw = ema_updates, semi_decay, teacher_loss_weight
+        self.nc, self.anchor_t, self.da_w = nc, anchor_t, da_loss_weight
+        self.cls_w = 0.3 * nc / 80. * 3. / len(STRIDES)
 
     def step(self, imgs, targets, u_strong, u_weak, Ms, conf_thres=0.1, iou_thres=0.65):
         H, W = u_weak.shape[2:]
@@ -61,12 +68,15 @@ class CpuSSODStep:
         n_img = imgs.shape[0]
         raw, feat = TrunkRef(self.student, self.depth, self.neck_depth, bn_momentum=self.bn_momentum).forward(torch.cat([imgs, u_strong], 0), train=True)
         sup_p, un_p = [r[:n_img] for r in raw], [r[n_img:] for r in raw]
-        sup_loss, _ = port.det_loss(sup_p, [port.build_targets(np.asarray(targets), ANCHORS_GRID, shapes)], [4.0, 1.0, 0.4], 0.05, 0.7, 0.3)
-        sup_loss = sup_loss + domain_focal([f[:n_img] for f in feat], 0) * 0 + domain_focal([f[n_img:] for f in feat], 1) * 0
+        sup_sets = [port.build_targets(np.asarray(targets), ANCHORS_GRID, shapes, self.anchor_t)]
+        sup_loss, _ = port.det_loss(sup_p, sup_sets, [4.0, 1.0, 0.4], 0.05, 0.7, self.cls_w)
+        sup_loss = sup_loss + domain_focal([f[:n_img] for f in feat], 0) * self.da_w + \
+            domain_focal([f[n_img:] for f in feat], 1) * self.da_w
         if len(rows):
-            sel = port.select_targets(rows, [0.6] * 80, [0.1] * 80, True)
-            sets = [port.build_targets(sel[0][:, :6], ANCHORS_GRID, shapes)] + [port.build_targets(s, ANCHORS_GRID, shapes, with_score=True) for s in sel[1:]]
-            un_loss, _ = port.det_loss(un_p, sets, [4.0, 1.0, 0.4], 0.05, 0.7, 0.3, with_bbox=True)
+            sel = port.select_targets(rows, [0.6] * self.nc, [0.1] * self.nc, True)
+            sets = [port.build_targets(sel[0][:, :6], ANCHORS_GRID, shapes, self.anchor_t)]
+            sets += [port.build_targets(s, ANCHORS_GRID, shapes, self.anchor_t, with_score=True) for s in sel[1:]]
+            un_loss, _ = port.det_loss(un_p, sets, [4.0, 1.0, 0.4], 0.05, 0.7, self.cls_w, with_bbox=True)
         else:
             un_loss = torch.zeros(1)
         loss = sup_loss + un_loss * self.tlw

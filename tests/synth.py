@@ -13,12 +13,13 @@ def level_shapes(img=640):
     return [(img // s, img // s) for s in STRIDES]
 
 
-def make_targets(seed, n, B, with_conf=False):
-    """[n,6] (img,cls,x,y,w,h) normalised; includes exact cell-boundary (.5) cases and same-cell duplicates."""
+def make_targets(seed, n, B, with_conf=False, nc=80):
+    """[n,6] (img,cls,x,y,w,h) normalised, classes in [0, nc); includes exact cell-boundary (.5) cases and same-cell
+    duplicates."""
     r = np.random.RandomState(seed)
     t = np.zeros((n, 6), F32)
     t[:, 0] = r.randint(0, B, n)
-    t[:, 1] = r.randint(0, 80, n)
+    t[:, 1] = r.randint(0, nc, n)
     t[:, 2:4] = r.uniform(0.1, 0.9, (n, 2))
     t[:, 4:6] = r.uniform(0.02, 0.32, (n, 2))
     k = n // 16
@@ -62,15 +63,47 @@ def make_Ms(seed, B, img=640):
     return Ms
 
 
-def make_pseudo_rows(seed, n, B):
-    """[n,9] float64 pseudo-label rows with confidences straddling the 0.1 / 0.6 / 0.99 thresholds."""
+def make_pseudo_rows(seed, n, B, nc=80):
+    """[n,9] float64 pseudo-label rows (classes in [0, nc)) with confidences straddling the 0.1 / 0.6 / 0.99 thresholds."""
     r = np.random.RandomState(seed)
-    t = make_targets(seed + 1, n, B).astype(np.float64)
+    t = make_targets(seed + 1, n, B, nc=nc).astype(np.float64)
     conf = r.uniform(0.02, 1.0, n)
     obj = np.where(r.uniform(size=n) < 0.3, r.uniform(0.99, 1.0, n), r.uniform(0.1, 1.0, n))
     cc = np.where(r.uniform(size=n) < 0.3, r.uniform(0.99, 1.0, n), r.uniform(0.1, 1.0, n))
     conf[:4] = [0.6, 0.1, np.float64(np.float32(0.6)), np.float64(np.float32(0.1))]   # exact-threshold cases
     return np.concatenate([t, conf[:, None], obj[:, None], cc[:, None]], 1)
+
+
+def make_teacher_pred_ties(seed, B, nc, ties, img=640):
+    """make_teacher_pred over every prediction of an img x img input at cand_frac 0.05; ties: class scores quantized to
+    quarters and candidate objectness to sixteenths, so the maximal class of a row is often shared (the first one wins) and
+    rows tie on confidence"""
+    P = sum(3 * ny * nx for ny, nx in level_shapes(img))
+    pred = make_teacher_pred(seed, B, P, nc=nc, cand_frac=0.05, img=img)
+    if ties:
+        pred[..., 5:] = np.round(pred[..., 5:] * 4) / 4
+        pred[..., 4] = np.where(pred[..., 4] > 0.1, np.round(pred[..., 4] * 16) / 16, pred[..., 4])
+    return pred
+
+
+def make_class_thresholds(nc):
+    """per-class (ignore_thres_high, ignore_thres_low) of ComputeStudentMatchLoss, not uniform across classes"""
+    r = np.random.RandomState(200 + nc)
+    return r.uniform(0.4, 0.8, nc), r.uniform(0.05, 0.3, nc)
+
+
+def make_pseudo_rows_dup(seed, n, B, nc=80):
+    """make_pseudo_rows whose first n/8 boxes come again with other confidences (duplicate cells across the routed sets),
+    sorted by image"""
+    rows = make_pseudo_rows(seed, n, B, nc=nc)
+    k = n // 8
+    rows[k:2 * k, :6] = rows[:k, :6]
+    return rows[np.argsort(rows[:, 0], kind="stable")]
+
+
+def grad_sample_idx(numel, level):
+    """the gradient elements the class-count loss fixtures store for one level"""
+    return np.random.RandomState(300 + level).randint(0, numel, 1024)
 
 
 def make_head_logits(seed, B, img=640, no=85, scale=1.5):

@@ -121,13 +121,15 @@ def test_rescale_matches_the_torch_op_path():
 
 # ---- run() against the composition of the oracles -----------------------------------------------------------------------
 
-def _detector(seed=0):
-    """A YOLOv5s SSOD model (outputs ((pred, raw), features)) whose head keeps classes 0..3 (objectness ~0.9) and pushes every other class below
-    conf_thres, so a val batch has a few hundred detections per image at conf 0.001"""
+def _detector(seed=0, nc=80):
+    """A YOLOv5s SSOD model (outputs ((pred, raw), features)) with nc classes whose head keeps classes 0..3 (objectness ~0.9)
+    and pushes every other class below conf_thres, so a val batch has a few hundred detections per image at conf 0.001"""
     from efficientteacher_b200.config import yolov5_ssod_cfg
     from efficientteacher_b200.model import Model
     torch.manual_seed(seed)
-    m = Model(yolov5_ssod_cfg('s', batch_size=4, img_size=160)).to(DEV)
+    cfg = yolov5_ssod_cfg('s', batch_size=4, img_size=160)
+    cfg.Dataset.nc, cfg.Dataset.names = nc, [str(i) for i in range(nc)]
+    m = Model(cfg).to(DEV)
     with torch.no_grad():
         for h in m.head.m:
             b = h.bias.view(3, -1)
@@ -137,9 +139,11 @@ def _detector(seed=0):
     return m.eval()
 
 
-def _loader(model, seed=3):
+def _loader(model, seed=3, single_cls=False):
     """three rect batches (H x W 128x160, 160x128, 128x128) of uint8 images; labels are jittered copies of a third of the
-    model's own detections (so every IoU threshold sees true positives) plus a few unmatched boxes"""
+    model's own detections (so every IoU threshold sees true positives) plus a few unmatched boxes; single_cls: every label
+    is class 0, as a single_cls dataset gives them"""
+    nc = model.nc
     from oracle import port
     from efficientteacher_b200 import val
     r = np.random.RandomState(seed)
@@ -157,14 +161,17 @@ def _loader(model, seed=3):
                 cx, cy, w, h = (x1 + x2) / 2 * j[0] ** 0.1, (y1 + y2) / 2 * j[1] ** 0.1, (x2 - x1) * j[2], (y2 - y1) * j[3]
                 rows.append((b, c, cx / W, cy / H, w / W, h / H))
             for _ in range(3):
-                rows.append((b, r.randint(0, 4), r.rand(), r.rand(), r.uniform(0.05, 0.3), r.uniform(0.05, 0.3)))
+                rows.append((b, r.randint(0, min(4, nc)), r.rand(), r.rand(), r.uniform(0.05, 0.3), r.uniform(0.05, 0.3)))
         tg = torch.tensor(rows, dtype=torch.float32).reshape(-1, 6)
+        if single_cls:
+            tg[:, 1] = 0
         batches.append((img, tg, ["im%d_%d.jpg" % (bi, b) for b in range(B)], _shapes(B, H, W, 10 + bi)))
     return batches
 
 
-def _composition(model, loader, nc=80):
-    """engine -> port.nms_val -> torch rescale -> port.process_batch -> ap_port.ap_per_class, then val.py:398-465"""
+def _composition(model, loader, nc=80, single_cls=False):
+    """engine -> port.nms_val -> torch rescale -> port.process_batch -> ap_port.ap_per_class, then val.py:398-465;
+    single_cls: class-agnostic NMS and every detection in class 0 (val.py:335-344), nc 1"""
     from oracle import port
     from efficientteacher_b200 import val
     iouv = torch.linspace(0.5, 0.95, 10).numpy()
@@ -173,7 +180,10 @@ def _composition(model, loader, nc=80):
         B, _, H, W = img.shape
         with torch.no_grad():
             pred = val._unwrap(model(img.to(DEV))[0])
-        dets = port.nms_val(pred.cpu().numpy(), 0.001, 0.6)
+        dets = port.nms_val(pred.cpu().numpy(), 0.001, 0.6, agnostic=single_cls)
+        if single_cls:
+            for d in dets:
+                d[:, 5] = 0
         t = tg.to(DEV).clone()
         t[:, 2:6] *= torch.tensor([W, H, W, H], device=DEV, dtype=torch.float32)
         for si, d in enumerate(dets):
@@ -212,6 +222,19 @@ def test_run_matches_the_composition_of_the_oracles():
     # as in the reference, an SSOD model without val_ssod unwraps to (pred, raw): not a prediction tensor
     with pytest.raises(TypeError):
         val.run({'nc': 80}, model=model, dataloader=loader, plots=False)
+
+
+@pytest.mark.parametrize("nc,single_cls", [(20, False), (2, False), (1, True)])
+def test_run_matches_the_composition_of_the_oracles_at_class_counts(nc, single_cls):
+    """run() at the class counts of VOC (20), the custom configs (2) and single_cls (a one-class model): ValEpoch's histogram
+    and etb_val_epoch_append / etb_ap_per_class sized by nc, the nc 1 NMS route, class-agnostic NMS with classes zeroed"""
+    from efficientteacher_b200 import val
+    model = _detector(nc=nc)
+    loader = _loader(model, single_cls=single_cls)
+    results, maps, _, cls_thr = val.run({'nc': nc}, model=model, dataloader=loader, plots=False, val_ssod=True, single_cls=single_cls)
+    want_results, want_maps, want_thr = _composition(model, loader, 1 if single_cls else nc, single_cls)
+    assert results == want_results and np.array_equal(maps, want_maps) and np.array_equal(cls_thr, want_thr), (results, want_results)
+    assert results[2] > 0.05 and len(maps) == (1 if single_cls else nc)
 
 
 def test_run_without_true_positives_returns_zeros():
