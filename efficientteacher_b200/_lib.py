@@ -114,17 +114,13 @@ _SIGS = {
                                    C.c_size_t, vp]),
     "etb_loss_backward": (C.c_int, [C.POINTER(vp), C.POINTER(vp), C.POINTER(EtbLossParams),
                                     C.POINTER(EtbAssignOut), vp, vp, C.c_size_t, vp]),
-    "etb_conv_workspace_bytes": (C.c_size_t, [C.POINTER(EtbConvParams)]),
-    "etb_conv_fwd": (C.c_int, [vp, vp, vp, vp, vp, vp, vp, C.POINTER(EtbConvParams), vp, C.c_size_t, vp]),
-    "etb_dgrad_weight_elems": (C.c_int64, [C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
-    "etb_pack_weight_dgrad": (C.c_int, [vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp]),
+    "etb_conv_fwd": (C.c_int, [vp, vp, vp, vp, vp, vp, vp, C.POINTER(EtbConvParams), vp]),
     "etb_conv_dgrad": (C.c_int, [vp, vp, vp, C.POINTER(EtbConvParams), C.c_int32, vp]),
     "etb_conv_wgrad_workspace_bytes": (C.c_size_t, [C.POINTER(EtbConvParams)]),
     "etb_conv_wgrad": (C.c_int, [vp, vp, vp, C.POINTER(EtbConvParams), C.c_int32, vp, C.c_size_t, vp]),
     "etb_bn_partial_rows": (C.c_int32, [C.c_int64, C.c_int32, C.c_int32]),
     "etb_bn_stats": (C.c_int, [vp, C.c_int64, C.c_int32, C.c_int32, vp, C.c_int32, vp]),
     "etb_bn_finalize": (C.c_int, [vp, C.c_int32, C.c_int64, C.c_int32, vp, vp, C.c_float, C.c_float, vp, vp, vp, vp, vp, vp, vp]),
-    "etb_bn_act_apply": (C.c_int, [vp, vp, vp, vp, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp]),
     "etb_bn_act_apply_res": (C.c_int, [vp, vp, vp, vp, vp, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp]),
     "etb_maxpool5_fwd": (C.c_int, [vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp]),
     "etb_maxpool5_bwd": (C.c_int, [vp, vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp]),
@@ -134,18 +130,14 @@ _SIGS = {
     "etb_bn_act_bwd_finalize": (C.c_int, [vp, C.c_int32, C.c_int32, vp, vp, vp, C.c_int32, vp]),
     "etb_bn_act_bwd_apply": (C.c_int, [vp, vp, vp, vp, vp, vp, vp, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                        vp, vp]),
-    "etb_stem_im2col": (C.c_int, [vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_float, vp]),
     "etb_nchw_f32_to_nhwc_bf16": (C.c_int, [vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                             C.c_float, vp]),
     "etb_nhwc_bf16_to_nchw_f32": (C.c_int, [vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp]),
     "etb_sppf_pool": (C.c_int, [vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp]),
     "etb_upsample2x_nhwc": (C.c_int, [vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                       C.c_int32, C.c_int32, vp]),
-    "etb_fold_bn": (C.c_int, [vp, vp, vp, vp, C.c_float, vp, vp, C.c_int32, vp]),
-    "etb_pack_weight": (C.c_int, [vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp]),
     "etb_pack_multi": (C.c_int, [vp, vp, C.c_int32, vp]),
     "etb_fold_bn_multi": (C.c_int, [vp, C.c_int32, vp]),
-    "etb_pack_stem_weight": (C.c_int, [vp, vp, C.c_int32, vp]),
     "etb_detect_dy_rows": (C.c_int64, [C.c_int32, C.c_int32, C.c_int32]),
     "etb_detect_dy_pack": (C.c_int, [vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp]),
     "etb_column_sum": (C.c_int, [vp, C.c_int64, C.c_int32, vp, C.c_int32, vp]),

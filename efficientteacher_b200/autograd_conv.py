@@ -382,7 +382,7 @@ def _conv_forward(ctx, x, weight, stride, pad, is_stem, wp, wd):
     Model.pack_weights(), else packed here."""
     Cout = weight.shape[0]
     if is_stem:
-        xs = x.im2col() if isinstance(x, StemInput) else co.stem_im2col(x.float(), 1.0)
+        xs = x.im2col() if isinstance(x, StemInput) else co.stem_im2col_parts([x], 255.0 if x.dtype == torch.uint8 else 1.0)
         xb, xcs, Cin, k, st, pd = xs, 128, 128, 1, 1, 0
         wp = co.pack_stem_weight(weight) if wp is None else wp
     else:
@@ -560,7 +560,7 @@ class NetDFn(torch.autograd.Function):
         if ctx.needs_input_grad[2]:
             dw2 = weight_grad(w2, lambda into: co.column_sum(partials, out=into, accumulate=True).view_as(w2))
         if ctx.needs_input_grad[0]:
-            wd = ctx.wd1n if ctx.wd1n is not None else co.pack_weight_dgrad(-w1.detach().float(), 1, 0)
+            wd = ctx.wd1n if ctx.wd1n is not None else co.pack_weight_dgrad(w1, 1, 0, negate=True)
             dx = input_grad(ctx.fan, lambda o, ocs, acc: co.conv_dgrad(dh, wd, N, H, W, C_, C_, 1, 1, 0, out=o, out_cstride=ocs,
                                                                        accumulate=acc), N, C_, H, W, g.device)
         if ctx.needs_input_grad[1]:

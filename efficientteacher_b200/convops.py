@@ -5,6 +5,7 @@ import torch
 
 from . import _lib
 from ._lib import EtbConvParams
+from .packing import WeightPacker
 
 # activation codes of the conv epilogue and the BatchNorm kernels (include/etb200.h); 3 is not a code
 ACT = {None: 0, "none": 0, "silu": 1, "relu": 2, "hard_swish": 4}
@@ -34,40 +35,26 @@ def to_nchw_f32(x_nhwc, C_=None, coffset=0):
     return y
 
 
-def pack_weight(w_oihw, cin_pad=None):
+def _pack_one(w_oihw, stride=1, pad=0, stem=False, dgrad=False, negate=False):
+    """packing.PackedConv of one weight, from a one-shot WeightPacker (the etb_pack_multi layouts).  The packer uploads its
+    descriptor table, which a stream capture does not allow: captured steps take their operands from Model.pack_weights."""
+    assert not torch.cuda.is_current_stream_capturing(), "one-shot weight packing inside a stream capture"
     w = w_oihw.detach().float().contiguous()
-    Cout, Cin, kh, kw = w.shape
-    cp = (Cin + 63) // 64 * 64 if cin_pad is None else cin_pad     # every tap padded to the 64-channel K block
-    out = torch.empty((Cout, kh * kw * cp), dtype=torch.bfloat16, device=w.device)
-    _lib.check(_lib.lib().etb_pack_weight(_lib.ptr(w), _lib.ptr(out), Cout, Cin, kh, kw, cp, _lib.stream_ptr()), "etb_pack_weight")
-    return out
+    pk = WeightPacker(w.device)
+    pc = pk.add(w, stride, pad, want_dgrad=dgrad, stem=stem, negate_dgrad=negate)
+    pk.run()
+    return pc
+
+
+def pack_weight(w_oihw):
+    """[Cout,Cin,k,k] -> forward operand [Cout][k*k*ceil64(Cin)] bf16: every tap padded to the 64-channel K block"""
+    return _pack_one(w_oihw).fwd
 
 
 def pack_stem_weight(w_oihw):
-    w = w_oihw.detach().float().contiguous()
-    assert tuple(w.shape[1:]) == (3, 6, 6)
-    out = torch.empty((w.shape[0], 128), dtype=torch.bfloat16, device=w.device)
-    _lib.check(_lib.lib().etb_pack_stem_weight(_lib.ptr(w), _lib.ptr(out), w.shape[0], _lib.stream_ptr()), "etb_pack_stem_weight")
-    return out
-
-
-def fold_bn(bn):
-    Cc = bn.weight.shape[0]
-    scale = torch.empty(Cc, dtype=torch.float32, device=bn.weight.device)
-    bias = torch.empty_like(scale)
-    _lib.check(_lib.lib().etb_fold_bn(_lib.ptr(bn.weight.detach()), _lib.ptr(bn.bias.detach()), _lib.ptr(bn.running_mean),
-                                      _lib.ptr(bn.running_var), float(bn.eps), _lib.ptr(scale), _lib.ptr(bias), Cc,
-                                      _lib.stream_ptr()), "etb_fold_bn")
-    return scale, bias
-
-
-def stem_im2col(x_nchw_f32, mul=1.0):
-    x = x_nchw_f32.float().contiguous()
-    N, Cc, H, W = x.shape
-    assert Cc == 3
-    out = nhwc_empty(N, H // 2, W // 2, 128, x.device)
-    _lib.check(_lib.lib().etb_stem_im2col(_lib.ptr(x), _lib.ptr(out), N, H, W, float(mul), _lib.stream_ptr()), "etb_stem_im2col")
-    return out
+    """[Cout,3,6,6] -> stem operand [Cout][128] bf16 in the stem_im2col_parts K order"""
+    assert tuple(w_oihw.shape[1:]) == (3, 6, 6)
+    return _pack_one(w_oihw, stem=True).fwd
 
 
 def _conv_params(N, H, W, Cin, Cout, k, stride, pad, **fields):
@@ -96,7 +83,7 @@ def conv_fwd(x, w_packed, Cin, Cout, k, stride, pad, scale=None, bias=None, act=
         cp.res_cstride, cp.res_coffset = residual.shape[3], res_coffset
     _lib.check(_lib.lib().etb_conv_fwd(C.c_void_p(xp), _lib.ptr(w_packed), _lib.ptr(scale), _lib.ptr(bias), _lib.ptr(residual),
                                        _lib.ptr(out) if det_out is None else C.c_void_p(0), _lib.ptr(det_out), C.byref(cp),
-                                       C.c_void_p(0), 0, _lib.stream_ptr()), "etb_conv_fwd")
+                                       _lib.stream_ptr()), "etb_conv_fwd")
     return out if det_out is None else det_out
 
 
@@ -115,14 +102,10 @@ def upsample2x(x, Cc, out, out_coffset, x_coffset=0, x_cstride=None):
     return out
 
 
-def pack_weight_dgrad(w_oihw, stride, pad):
-    w = w_oihw.detach().float().contiguous()
-    Cout, Cin, k, _ = w.shape
-    n = int(_lib.lib().etb_dgrad_weight_elems(Cout, Cin, k, stride))
-    out = torch.empty(n, dtype=torch.bfloat16, device=w.device)
-    _lib.check(_lib.lib().etb_pack_weight_dgrad(_lib.ptr(w), _lib.ptr(out), Cout, Cin, k, stride, pad, _lib.stream_ptr()),
-               "etb_pack_weight_dgrad")
-    return out
+def pack_weight_dgrad(w_oihw, stride, pad, negate=False):
+    """[Cout,Cin,k,k] -> the etb_conv_dgrad operand: per parity class (packing.dgrad_classes) a [Cin][ntaps][ceil64(Cout)]
+    bf16 block, concatenated (Cin*k*k*ceil64(Cout) elements).  negate: the operand of -W (a conv behind GradReverse)."""
+    return _pack_one(w_oihw, stride, pad, dgrad=True, negate=negate).dgrad
 
 
 def conv_dgrad(dy, wd_packed, N, H, W, Cin, Cout, k, stride, pad, out=None, out_coffset=0, dy_coffset=0, accumulate=False,

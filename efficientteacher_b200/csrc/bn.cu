@@ -488,10 +488,6 @@ extern "C" int etb_bn_act_apply_res(const void* y_bf16, const float* scale, cons
   ETB_CHECK_LAUNCH();
   return ETB_OK;
 }
-extern "C" int etb_bn_act_apply(const void* y_bf16, const float* scale, const float* shift, void* out_bf16, int64_t M, int32_t C,
-                                int32_t y_cstride, int32_t out_cstride, int32_t act, void* stream) {
-  return etb_bn_act_apply_res(y_bf16, scale, shift, nullptr, out_bf16, M, C, y_cstride, 0, out_cstride, act, stream);
-}
 
 // partials: [rows = etb_bn_partial_rows(M,C,1)][2][C] floats: per-block [sum dz][sum dz*xhat], fully overwritten
 extern "C" int etb_bn_act_bwd_reduce(const void* da_bf16, const void* y_bf16, const float* scale, const float* shift, const float* mean,

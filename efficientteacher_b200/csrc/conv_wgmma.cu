@@ -508,7 +508,7 @@ static int launch_gemm(const GemmGeom& g, ConvKArgs ka, cudaStream_t st) {
     return ETB_ERR_CUDA;
   }
   // aC need not be a multiple of the 64-channel K block: the A box is clipped by TMA (zero fill beyond aC) and the B operand is
-  // packed with every tap padded to aCp = ceil64(aC) zero columns (etb_pack_weight Cin_pad / dgrad out_ld)
+  // packed with every tap padded to aCp = ceil64(aC) zero columns (etb_pack_multi mode 0 / mode 1 out_ld)
   ETB_CHECK_ARG(g.aC % 8 == 0 && g.aC > 0 && g.a_cstride >= g.aC && g.a_cstride % 8 == 0);
   const int aCp = (g.aC + CONV_BLOCK_K - 1) / CONV_BLOCK_K * CONV_BLOCK_K;
   ETB_CHECK_ARG((((uintptr_t)g.a_ptr) & 15) == 0 && (((uintptr_t)g.b_ptr) & 15) == 0);
@@ -570,12 +570,8 @@ static int launch_gemm(const GemmGeom& g, ConvKArgs ka, cudaStream_t st) {
   return BN == 128 ? launch_conv<128>(mA, mB, ka, grid, st) : launch_conv<64>(mA, mB, ka, grid, st);
 }
 
-extern "C" size_t etb_conv_workspace_bytes(const EtbConvParams* cp) { (void)cp; return 0; }
-
 extern "C" int etb_conv_fwd(const void* x_bf16, const void* w_bf16, const float* scale, const float* bias,
-                            const void* residual_bf16, void* y_bf16, float* y_f32, const EtbConvParams* cp, void* workspace,
-                            size_t workspace_bytes, void* stream) {
-  (void)workspace; (void)workspace_bytes;
+                            const void* residual_bf16, void* y_bf16, float* y_f32, const EtbConvParams* cp, void* stream) {
   ETB_CHECK_ARG(x_bf16 && w_bf16 && cp && (y_bf16 || y_f32));
   ETB_CHECK_ARG(cp->N > 0 && cp->H > 0 && cp->W > 0 && cp->Cin > 0 && cp->Cout > 0);
   ETB_CHECK_ARG(cp->act == 0 || cp->act == 1 || cp->act == 2 || cp->act == 4);
@@ -618,59 +614,20 @@ extern "C" int etb_conv_fwd(const void* x_bf16, const void* w_bf16, const float*
 // ---- data gradient (K2): dx = conv_transpose(dy, W) as implicit GEMMs on the same kernel ------------------------------
 // For each output-parity class (ph,pw) of dx (one class when stride==1):  dx[n, s*i+ph, s*j+pw, :] =
 //   sum over the taps (kh,kw) with (ph+pad-kh) % s == 0, (pw+pad-kw) % s == 0 of  dy[n, i+dh, j+dw, :] * W[:, :, kh, kw]
-//   with dh = (ph+pad-kh)/s, dw = (pw+pad-kw)/s.   B operand: etb_pack_weight_dgrad (same tap order).
-static int dgrad_taps(int k, int s, int pad, int ph, int pw, signed char* kh_l, signed char* kw_l, signed char* dh, signed char* dw) {
+//   with dh = (ph+pad-kh)/s, dw = (pw+pad-kw)/s.   B operand: etb_pack_multi mode 1 (or 3), one block per class in this
+//   class and tap order (packing.dgrad_classes), each [Cin][ntaps][ceil64(Cout)].
+static int dgrad_taps(int k, int s, int pad, int ph, int pw, signed char* dh, signed char* dw) {
   int n = 0;
   for (int kh = 0; kh < k; ++kh) {
     if ((ph + pad - kh) % s != 0) continue;
     for (int kw = 0; kw < k; ++kw) {
       if ((pw + pad - kw) % s != 0) continue;
-      kh_l[n] = (signed char)kh; kw_l[n] = (signed char)kw;
       // floor division is exact here (remainder checked); C division of negatives truncates toward zero, also exact
       dh[n] = (signed char)((ph + pad - kh) / s); dw[n] = (signed char)((pw + pad - kw) / s);
       ++n;
     }
   }
   return n;
-}
-
-extern "C" int64_t etb_dgrad_weight_elems(int32_t Cout, int32_t Cin, int32_t k, int32_t stride) {
-  (void)stride;
-  const int64_t Coutp = (Cout + CONV_BLOCK_K - 1) / CONV_BLOCK_K * CONV_BLOCK_K;   // every tap padded to the 64-channel K block
-  return (int64_t)Cin * k * k * Coutp;   // all parity classes together visit every tap exactly once
-}
-
-struct TapTable { signed char v[24]; };
-__global__ void __launch_bounds__(256) pack_weight_dgrad_kernel(const float* __restrict__ w, __nv_bfloat16* __restrict__ o, int Cout, int Coutp, int Cin, int k, int ntaps, TapTable tt) {
-  const int64_t total = (int64_t)Cin * ntaps * Coutp;
-  for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (int64_t)gridDim.x * blockDim.x) {
-    const int co = (int)(e % Coutp);
-    const int t = (int)((e / Coutp) % ntaps);
-    const int ci = (int)(e / ((int64_t)Coutp * ntaps));
-    o[e] = __float2bfloat16(co < Cout ? w[(((int64_t)co * Cin + ci) * k + tt.v[t]) * k + tt.v[12 + t]] : 0.f);
-  }
-}
-
-// w [Cout,Cin,k,k] fp32 -> for each parity class c (row-major ph,pw) a [Cin][ntaps_c*ceil64(Cout)] bf16 block (zero padded), blocks concatenated
-extern "C" int etb_pack_weight_dgrad(const float* w_oihw, void* out_bf16, int32_t Cout, int32_t Cin, int32_t k, int32_t stride,
-                                     int32_t pad, void* stream) {
-  ETB_CHECK_ARG(w_oihw && out_bf16 && Cout > 0 && Cin > 0 && k >= 1 && k * k <= 12 && (stride == 1 || stride == 2));
-  __nv_bfloat16* o = (__nv_bfloat16*)out_bf16;
-  for (int ph = 0; ph < stride; ++ph)
-    for (int pw = 0; pw < stride; ++pw) {
-      TapTable tt;
-      signed char dh[12], dw[12];
-      const int nt = dgrad_taps(k, stride, pad, ph, pw, tt.v, tt.v + 12, dh, dw);
-      if (nt == 0) continue;
-      const int Coutp = (Cout + CONV_BLOCK_K - 1) / CONV_BLOCK_K * CONV_BLOCK_K;
-      const int64_t total = (int64_t)Cin * nt * Coutp;
-      int64_t blocks = (total + 255) / 256;
-      if (blocks > etb_num_sms() * 16) blocks = etb_num_sms() * 16;
-      etb_launch(pack_weight_dgrad_kernel, dim3((unsigned)blocks), dim3(256), 0, (cudaStream_t)stream, w_oihw, o, Cout, Coutp, Cin, k, nt, tt);
-      ETB_CHECK_LAUNCH();
-      o += total;
-    }
-  return ETB_OK;
 }
 
 // dy [N,Ho,Wo,*] bf16 (channels [dy_coffset.. +Cout) of stride dy_cstride) -> dx [N,H,W,*] bf16 at channel offset.
@@ -690,9 +647,8 @@ extern "C" int etb_conv_dgrad(const void* dy_bf16, const void* wd_bf16, void* dx
     for (int pw = 0; pw < s; ++pw) {
       ConvKArgs ka;
       memset(&ka, 0, sizeof(ka));
-      signed char kh_l[12], kw_l[12];
-      const int nt = dgrad_taps(k, s, pad, ph, pw, kh_l, kw_l, ka.tap_dh, ka.tap_dw);
-      // etb_pack_weight_dgrad packs a block for every class with taps, also for classes with no pixels (H or W == 1):
+      const int nt = dgrad_taps(k, s, pad, ph, pw, ka.tap_dh, ka.tap_dw);
+      // the operand holds a block for every class with taps, also for classes with no pixels (H or W == 1):
       // step past it before skipping the class, or the next class would run on this one's weights
       const __nv_bfloat16* wcls = wd;
       wd += (size_t)cp->Cin * nt * Coutp;

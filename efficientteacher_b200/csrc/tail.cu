@@ -303,11 +303,15 @@ extern "C" int etb_domain_focal_bwd(const EtbFocalParams* fp, const float* gout,
   return ETB_OK;
 }
 
-// ------------------------------------------------------------------------------------------------ stem im2col from uint8
-// Same tiling as stem_im2col_kernel (trunk.cu): K order (c,kh,kw), 64 output pixels of one output row per block.  The input
-// is the loaders' uint8 NCHW batch; value = float(u8) / 255 (IEEE division: bit-identical to `.float() / 255`), rounded
-// to bf16 once.  Several source batches (labeled, strong-aug) are written into one im2col buffer at an image offset, which
-// is the student's torch.cat((imgs, unlabeled_imgs), 0) (ssod_trainer.py:620) without the copy.
+// ------------------------------------------------------------------------------------------------ stem im2col
+// 6x6 s2 p2 over 3 channels -> K = 128 slots, 108 used.  K order k = (c*6 + kh)*6 + kw, i.e. exactly the [ci][kh][kw] order
+// of the OIHW weight row, so the weight pack is a copy.  One block = 64 consecutive output pixels of one output row: the
+// 18 (c,kh) input row segments (132 values each) are staged in shared memory with coalesced loads (zero-filled outside the
+// image = the conv padding), then every thread assembles 16 B chunks [pixel][8 k] so a warp writes 512 contiguous bytes.
+// The input is the loaders' uint8 NCHW batch (div 255) or an fp32 one (div 1); value = float(x) / div (IEEE division:
+// bit-identical to `.float() / 255`, and exact for div 1), rounded to bf16 once.  Several source batches (labeled,
+// strong-aug) are written into one im2col buffer at an image offset, which is the student's
+// torch.cat((imgs, unlabeled_imgs), 0) (ssod_trainer.py:620) without the copy.
 #define STEM_TP 64
 #define STEM_PITCH 133
 template <typename T>

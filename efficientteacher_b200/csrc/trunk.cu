@@ -1,5 +1,4 @@
 // trunk.cu -- layout / pooling / folding helpers around the wgmma convolutions (K3, K4, K18).
-//   stem im2col + /255      reference trainer/ssod_trainer.py:694-696, models/backbone/yolov5_backbone.py:56
 //   SPPF max pools + concat reference models/backbone/common.py:702-708
 //   nearest 2x upsample     reference models/neck/yolov5_neck.py:92,97 (+ Concat common.py:796-797, free by slicing)
 //   eval BN folding         reference utils/torch_utils.py:199-219 (fuse_conv_and_bn algebra), bn eps 1e-3
@@ -10,64 +9,6 @@ static inline unsigned grid_for(int64_t n, int threads) {
   int64_t b = (n + threads - 1) / threads;
   const int64_t cap = (int64_t)etb_num_sms() * 32;
   return (unsigned)(b > cap ? cap : (b < 1 ? 1 : b));
-}
-
-// ---- stem im2col (6x6 s2 p2, 3 channels -> K = 128 slots, 108 used) ----
-// K order k = (c*6 + kh)*6 + kw, i.e. exactly the [ci][kh][kw] order of the OIHW weight row, so the weight pack is a copy.
-// One block = 64 consecutive output pixels of one output row: the 18 (c,kh) input row segments (132 floats each) are
-// staged in shared memory with coalesced loads (zero-filled outside the image = the conv padding), then every thread
-// assembles 16 B chunks [pixel][8 k] so a warp writes 512 contiguous bytes.  HBM-bound: 12 B/pixel-channel read
-// (L2 serves the 3x row overlap), 256 B/pixel written.
-#define STEM_TP 64
-#define STEM_PITCH 133
-__global__ void __launch_bounds__(256) stem_im2col_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ y, int N, int H, int W, float mul) {
-  __shared__ float sm[18 * STEM_PITCH];
-  const int Ho = H / 2, Wo = W / 2;
-  const int tiles_w = (Wo + STEM_TP - 1) / STEM_TP;
-  const int tw = blockIdx.x % tiles_w;
-  const int oh = (blockIdx.x / tiles_w) % Ho;
-  const int n = blockIdx.x / (tiles_w * Ho);
-  const int ow0 = tw * STEM_TP;
-  const int iw0 = 2 * ow0 - 2, ih0 = 2 * oh - 2;
-  for (int i = threadIdx.x; i < 18 * 132; i += 256) {
-    const int row = i / 132, col = i - row * 132;
-    const int c = row / 6, kh = row - c * 6;
-    const int ih = ih0 + kh, iw = iw0 + col;
-    float v = 0.f;
-    if (ih >= 0 && ih < H && iw >= 0 && iw < W) v = __fmul_rn(__ldg(x + (((int64_t)n * 3 + c) * H + ih) * W + iw), mul);
-    sm[row * STEM_PITCH + col] = v;
-  }
-  __syncthreads();
-  const int g = threadIdx.x & 15;          // the 8-element K group is fixed per thread
-  int off[8];
-#pragma unroll
-  for (int j = 0; j < 8; ++j) {
-    const int k = g * 8 + j;
-    off[j] = k < 108 ? (k / 6) * STEM_PITCH + (k % 6) : -1;
-  }
-  uint4* yo = reinterpret_cast<uint4*>(y) + (((int64_t)n * Ho + oh) * Wo + ow0) * 16;
-#pragma unroll
-  for (int q = threadIdx.x; q < STEM_TP * 16; q += 256) {
-    const int pp = q >> 4;
-    if (ow0 + pp >= Wo) break;
-    float f[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) f[j] = off[j] >= 0 ? sm[off[j] + 2 * pp] : 0.f;
-    uint4 ov;
-    __nv_bfloat162* o = reinterpret_cast<__nv_bfloat162*>(&ov);
-#pragma unroll
-    for (int j = 0; j < 4; ++j) o[j] = __floats2bfloat162_rn(f[2 * j], f[2 * j + 1]);
-    yo[q] = ov;
-  }
-}
-
-extern "C" int etb_stem_im2col(const float* x, void* y_bf16, int32_t N, int32_t H, int32_t W, float mul, void* stream) {
-  ETB_CHECK_ARG(x && y_bf16 && N > 0 && H > 0 && W > 0 && H % 2 == 0 && W % 2 == 0);
-  const int64_t blocks = (int64_t)N * (H / 2) * ((W / 2 + STEM_TP - 1) / STEM_TP);
-  ETB_CHECK_ARG(blocks < (1ll << 31));
-  etb_launch(stem_im2col_kernel, dim3((unsigned)blocks), dim3(256), 0, (cudaStream_t)stream, x, (__nv_bfloat16*)y_bf16, N, H, W, mul);
-  ETB_CHECK_LAUNCH();
-  return ETB_OK;
 }
 
 // ---- NCHW fp32 <-> NHWC bf16 (simple gather; used at the edges of the trunk and by the tests) ----
@@ -167,57 +108,10 @@ extern "C" int etb_upsample2x_nhwc(const void* x_bf16, void* y_bf16, int32_t N, 
   return ETB_OK;
 }
 
-// ---- BN folding + weight packing ----
-__global__ void fold_bn_kernel(const float* g, const float* b, const float* m, const float* v, float eps, float* scale, float* bias, int C) {
-  const int c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c >= C) return;
-  const float s = g[c] / sqrtf(v[c] + eps);
-  scale[c] = s;
-  bias[c] = b[c] - m[c] * s;
-}
-extern "C" int etb_fold_bn(const float* gamma, const float* beta, const float* mean, const float* var, float eps, float* scale,
-                           float* bias, int32_t C, void* stream) {
-  ETB_CHECK_ARG(gamma && beta && mean && var && scale && bias && C > 0);
-  etb_launch(fold_bn_kernel, dim3((C + 127) / 128), dim3(128), 0, (cudaStream_t)stream, gamma, beta, mean, var, eps, scale, bias, C);
-  ETB_CHECK_LAUNCH();
-  return ETB_OK;
-}
-
-__global__ void __launch_bounds__(256) pack_weight_kernel(const float* __restrict__ w, __nv_bfloat16* __restrict__ o, int Cout, int Cin, int kh, int kw, int Cp) {
-  const int64_t total = (int64_t)Cout * kh * kw * Cp;
-  for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (int64_t)gridDim.x * blockDim.x) {
-    const int c = (int)(e % Cp);
-    const int64_t t = e / Cp;
-    const int x = (int)(t % kw), y = (int)((t / kw) % kh), oc = (int)(t / ((int64_t)kw * kh));
-    o[e] = __float2bfloat16(c < Cin ? w[(((int64_t)oc * Cin + c) * kh + y) * kw + x] : 0.f);
-  }
-}
-extern "C" int etb_pack_weight(const float* w_oihw, void* w_bf16, int32_t Cout, int32_t Cin, int32_t kh, int32_t kw, int32_t Cin_pad, void* stream) {
-  ETB_CHECK_ARG(w_oihw && w_bf16 && Cout > 0 && Cin > 0 && kh > 0 && kw > 0 && Cin_pad >= Cin);
-  etb_launch(pack_weight_kernel, dim3(grid_for((int64_t)Cout * kh * kw * Cin_pad, 256)), dim3(256), 0, (cudaStream_t)stream, w_oihw, (__nv_bfloat16*)w_bf16, Cout, Cin, kh, kw, Cin_pad);
-  ETB_CHECK_LAUNCH();
-  return ETB_OK;
-}
-
-__global__ void pack_stem_weight_kernel(const float* __restrict__ w, __nv_bfloat16* __restrict__ o, int Cout) {
-  const int e = blockIdx.x * blockDim.x + threadIdx.x;
-  if (e >= Cout * 128) return;
-  const int k = e & 127, oc = e >> 7;
-  float v = 0.f;
-  if (k < 108) v = w[oc * 108 + k];          // K order (c,kh,kw) == the OIHW row
-  o[e] = __float2bfloat16(v);
-}
-extern "C" int etb_pack_stem_weight(const float* w_oihw, void* w_bf16, int32_t Cout, void* stream) {
-  ETB_CHECK_ARG(w_oihw && w_bf16 && Cout > 0);
-  etb_launch(pack_stem_weight_kernel, dim3((Cout * 128 + 255) / 256), dim3(256), 0, (cudaStream_t)stream, w_oihw, (__nv_bfloat16*)w_bf16, Cout);
-  ETB_CHECK_LAUNCH();
-  return ETB_OK;
-}
-
-// ---- multi-tensor weight packing / BN folding: ONE launch for all ~104 convs of the trunk (replaces ~440 tiny launches/step) ----
+// ---- weight packing / BN folding: ONE launch for all ~104 convs of the trunk (also the packer of a single weight) ----
 // mode 0: fwd  [Cout][kh][kw][Cin or out_ld]   <- w[co][ci][kh][kw]        (dst index e: ci fastest; out_ld > Cin pads every tap)
 // mode 1: dgrad class  [Cin][ntaps][out_ld>=Cout] <- w[co][ci][kh_t][kw_t]   (dst: co fastest; row pitch out_ld per tap)
-// mode 2: stem [Cout][128] in the etb_stem_im2col K order
+// mode 2: stem [Cout][128] in the etb_stem_im2col_into K order (c,kh,kw) = the OIHW row, zero above 108
 // mode 3: mode 1 negated (dgrad operand of a conv that sits behind a GradReverse)
 __global__ void __launch_bounds__(256) pack_multi_kernel(const EtbPackDesc* __restrict__ descs, const int2* __restrict__ chunks) {
   const int2 ch = chunks[blockIdx.x];

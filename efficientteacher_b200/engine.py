@@ -122,7 +122,7 @@ class TrunkEngine:
         cat4 = co.nhwc_empty(N, H // 32, W // 32, nk.output_p4 + half5, dev)  # [conv4(x3), xp_1]   :106
         # backbone (yolov5_backbone.py:76-88)
         # uint8 = the loaders' raw batch (value / 255 inside the im2col kernel); fp32 = the reference contract (already scaled)
-        col = co.stem_im2col_parts([x], 255.0) if x.dtype == torch.uint8 else co.stem_im2col(x, 1.0)
+        col = co.stem_im2col_parts([x], 255.0 if x.dtype == torch.uint8 else 1.0)
         self.launches += 1
         x1 = self._conv("backbone.stage1", col, cin=128)
         x21 = self._conv("backbone.stage2_1", x1)

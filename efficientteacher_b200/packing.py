@@ -44,11 +44,11 @@ class PackedConv:
 class WeightPacker:
     def __init__(self, device):
         self.device = device
-        self.items = []          # (weight tensor, PackedConv, kind, cout_pad)
+        self.items = []          # (weight tensor, PackedConv, kind)
         self.folds = []          # (bn module, PackedConv)
         self._built = None
 
-    def add(self, weight, stride, pad, want_dgrad, stem=False, dgrad_cout_pad=None, negate_dgrad=False):
+    def add(self, weight, stride, pad, want_dgrad, stem=False, negate_dgrad=False):
         Cout, Cin, k, _ = weight.shape
         pc = PackedConv()
         pc.Cin, pc.Cout, pc.k, pc.s, pc.p = (128 if stem else Cin), Cout, (1 if stem else k), (1 if stem else stride), (0 if stem else pad)
@@ -56,10 +56,9 @@ class WeightPacker:
         pc.fwd = torch.zeros((Cout, 128 if stem else k * k * _ceil64(Cin)), dtype=torch.bfloat16, device=self.device)
         pc.dgrad = None
         if want_dgrad and not stem:
-            ld = _ceil64(Cout) if dgrad_cout_pad is None else dgrad_cout_pad
-            pc.dgrad = torch.zeros(Cin * k * k * ld, dtype=torch.bfloat16, device=self.device)
+            pc.dgrad = torch.zeros(Cin * k * k * _ceil64(Cout), dtype=torch.bfloat16, device=self.device)
         pc.scale = pc.bias = None
-        self.items.append((weight, pc, "stem" if stem else ("conv_neg" if negate_dgrad else "conv"), dgrad_cout_pad))
+        self.items.append((weight, pc, "stem" if stem else ("conv_neg" if negate_dgrad else "conv")))
         self._built = None
         return pc
 
@@ -83,14 +82,14 @@ class WeightPacker:
             for c in range((elems + ETB_PACK_CHUNK - 1) // ETB_PACK_CHUNK):
                 chunks.append((idx, c))
 
-        for w, pc, kind, cpad in self.items:
+        for w, pc, kind in self.items:
             Cout, Cin, k, _ = w.shape
             if kind == "stem":
                 push(w, pc.fwd.data_ptr(), Cout * 128, Cout, 3, 6, 2)
                 continue
             push(w, pc.fwd.data_ptr(), Cout * k * k * Cin, Cout, Cin, k, 0, out_ld=_ceil64(Cin))
             if pc.dgrad is not None:
-                ld = _ceil64(Cout) if cpad is None else cpad
+                ld = _ceil64(Cout)
                 off = 0
                 for khs, kws in dgrad_classes(k, pc.s, pc.p):
                     nt = len(khs)

@@ -249,18 +249,14 @@ typedef struct EtbConvParams {
   int32_t det_no;                          /* y_f32 path: outputs per anchor (85); Cout = na*det_no */
 } EtbConvParams;
 
-size_t etb_conv_workspace_bytes(const EtbConvParams* cp);
 int etb_conv_fwd(const void* x_bf16, const void* w_bf16, const float* scale, const float* bias,
-                 const void* residual_bf16, void* y_bf16, float* y_f32, const EtbConvParams* cp,
-                 void* workspace, size_t workspace_bytes, void* stream);
+                 const void* residual_bf16, void* y_bf16, float* y_f32, const EtbConvParams* cp, void* stream);
 
 /* data gradient of the same convolution (autograd of Conv.forward, SURVEY.md K2): dx = conv_transpose(dy, W), run as
  * implicit GEMMs on the same wgmma kernel -- one launch per output-parity class (1 for stride 1, 4 for stride 2).
  * `cp` describes the FORWARD conv; cp->x_cstride is the channel stride of dy, cp->y_cstride / y_coffset place dx.
- * wd = etb_pack_weight_dgrad(w) (etb_dgrad_weight_elems bf16 elements).  accumulate != 0: dx += result. */
-int64_t etb_dgrad_weight_elems(int32_t Cout, int32_t Cin, int32_t k, int32_t stride);
-int etb_pack_weight_dgrad(const float* w_oihw, void* out_bf16, int32_t Cout, int32_t Cin, int32_t k, int32_t stride,
-                          int32_t pad, void* stream);
+ * wd = the etb_pack_multi mode 1 (or 3) blocks of every parity class, concatenated: Cin*k*k*ceil64(Cout) bf16 elements.
+ * accumulate != 0: dx += result. */
 int etb_conv_dgrad(const void* dy_bf16, const void* wd_bf16, void* dx_bf16, const EtbConvParams* cp, int32_t accumulate,
                    void* stream);
 
@@ -269,7 +265,7 @@ int etb_conv_dgrad(const void* dy_bf16, const void* wd_bf16, void* dx_bf16, cons
  * partial tile into its slice of `workspace`, then a reduce kernel sums the slices, converts to the parameter layout
  * [Cout,Cin,kh,kw] and writes (flags bit1: adds into) dw_f32 -- which may be the gradient-arena slice of the parameter.
  * `cp` describes the FORWARD conv; cp->x_cstride is x's channel stride, cp->y_cstride dy's.
- * flags bit0: stem (cp = the K=128 pointwise GEMM over the etb_stem_im2col buffer; dw_f32 is [Cout,3,6,6]). */
+ * flags bit0: stem (cp = the K=128 pointwise GEMM over the etb_stem_im2col_into buffer; dw_f32 is [Cout,3,6,6]). */
 size_t etb_conv_wgrad_workspace_bytes(const EtbConvParams* cp);
 int etb_conv_wgrad(const void* x_bf16, const void* dy_bf16, float* dw_f32, const EtbConvParams* cp, int32_t flags,
                    void* workspace, size_t workspace_bytes, void* stream);
@@ -281,7 +277,7 @@ int etb_conv_wgrad(const void* x_bf16, const void* dy_bf16, float* dw_f32, const
  * for -3 < z < 3, 1 for z >= 3: torch's hardswish_backward); any other value is ETB_ERR_INVALID.
  *   forward : etb_bn_stats (per-block partial rows [rows][2][C] = sum y, sum y^2; rows = etb_bn_partial_rows(M,C,0))
  *             -> etb_bn_finalize (fixed-order sum of the rows -> scale, shift, mean, invstd, running stats)
- *             -> etb_bn_act_apply (a = act(y*scale+shift))
+ *             -> etb_bn_act_apply_res (a = act(y*scale+shift) [+ res])
  *   backward: etb_bn_act_bwd_reduce (partial rows of sum dz, sum dz*xhat; dz = da*act'(z); rows = etb_bn_partial_rows(M,C,1))
  *             -> etb_bn_act_bwd_finalize (sums[2C]; dbeta, dgamma written or accumulated into the parameters' .grad)
  *             -> etb_bn_act_bwd_apply (dy = gamma*invstd*(dz - sum_dz/M - xhat*sum_dz_xhat/M))
@@ -291,10 +287,8 @@ int etb_bn_stats(const void* y_bf16, int64_t M, int32_t C, int32_t y_cstride, fl
 int etb_bn_finalize(const float* partials, int32_t rows, int64_t M, int32_t C, const float* gamma, const float* beta, float eps,
                     float momentum, float* running_mean, float* running_var, float* scale, float* shift, float* mean,
                     float* invstd, void* stream);
-int etb_bn_act_apply(const void* y_bf16, const float* scale, const float* shift, void* out_bf16, int64_t M, int32_t C,
-                     int32_t y_cstride, int32_t out_cstride, int32_t act, void* stream);
-/* same + the Bottleneck shortcut (models/backbone/common.py:499 `x + cv2(cv1(x))`): out = act(y*scale+shift) + res
- * (res may be NULL; res is NHWC bf16 with its own channel stride) */
+/* out = act(y*scale+shift), + res when res != NULL: the Bottleneck shortcut (models/backbone/common.py:499
+ * `x + cv2(cv1(x))`); res is NHWC bf16 with its own channel stride */
 int etb_bn_act_apply_res(const void* y_bf16, const float* scale, const float* shift, const void* res_bf16, void* out_bf16,
                          int64_t M, int32_t C, int32_t y_cstride, int32_t res_cstride, int32_t out_cstride, int32_t act,
                          void* stream);
@@ -309,10 +303,6 @@ int etb_bn_act_bwd_apply(const void* da_bf16, const void* y_bf16, const float* s
 
 /* small layout / elementwise helpers of the trunk (all HBM-bound, coalesced 16 B vectors) */
 
-/* input prep + stem im2col (trainer/ssod_trainer.py:694-696 `.float()/255` fused with the 6x6 s2 p2 stem patch
- * gather of models/backbone/yolov5_backbone.py:56): x [N,3,H,W] fp32 NCHW -> y [N,H/2,W/2,128] bf16 with
- * K index (c*6+kh)*6+kw (the OIHW weight row order) for K<108 and zeros above; `mul` scales the pixels (1/255 for uint8-range input, else 1). */
-int etb_stem_im2col(const float* x, void* y_bf16, int32_t N, int32_t H, int32_t W, float mul, void* stream);
 /* NCHW fp32 <-> NHWC bf16 (channel stride / offset on the NHWC side) */
 int etb_nchw_f32_to_nhwc_bf16(const float* x, void* y, int32_t N, int32_t C, int32_t H, int32_t W,
                               int32_t y_cstride, int32_t y_coffset, float mul, void* stream);
@@ -340,16 +330,13 @@ int etb_upsample2x_bwd(const void* dy_bf16, void* dx_bf16, int32_t N, int32_t H,
                        int32_t dx_cstride, void* stream);
 int etb_copy_slice_nhwc(const void* x_bf16, void* y_bf16, int64_t M, int32_t C, int32_t x_cstride, int32_t y_cstride,
                         void* stream);
-/* eval-mode BatchNorm folded to per-channel scale/bias: scale = g/sqrt(var+eps), bias = b - mean*scale */
-int etb_fold_bn(const float* gamma, const float* beta, const float* mean, const float* var, float eps,
-                float* scale, float* bias, int32_t C, void* stream);
-/* conv weight [Cout,Cin,kh,kw] fp32 -> [Cout][kh][kw][Cin_pad] bf16 (K-major GEMM operand), zero padded */
-int etb_pack_weight(const float* w_oihw, void* w_bf16, int32_t Cout, int32_t Cin, int32_t kh, int32_t kw,
-                    int32_t Cin_pad, void* stream);
-/* multi-tensor variants: one launch packs every conv weight of the model (descs and the chunk list live in device memory;
- * chunk = {desc index, chunk index} covering ETB_PACK_CHUNK destination elements).  mode 0: forward operand
- * [Cout][kh][kw][Cin]; mode 1: one dgrad parity class [Cin][ntaps][out_ld] (tap t = (kh[t],kw[t])); mode 2: stem [Cout][128];
- * mode 3: mode 1 with the sign flipped (dgrad operand of a conv behind GradReverse, models/detector/yolo_ssod.py:158-172). */
+/* conv weight packing: one launch packs every conv weight of the model, or a single one (descs and the chunk list live in
+ * device memory; chunk = {desc index, chunk index} covering ETB_PACK_CHUNK destination elements).  w [Cout,Cin,k,k] fp32 ->
+ * bf16 K-major GEMM operands, written only at real elements (the caller zeroes the pads):
+ *   mode 0: forward operand [Cout][kh][kw][out_ld], out_ld = Cin or ceil64(Cin) (every tap padded to the 64-channel K block);
+ *   mode 1: one dgrad parity class [Cin][ntaps][out_ld >= Cout] (tap t = (kh[t],kw[t]));
+ *   mode 2: stem [Cout][128] in the etb_stem_im2col_into K order (c*6+kh)*6+kw = the OIHW row, zero above 108;
+ *   mode 3: mode 1 with the sign flipped (dgrad operand of a conv behind GradReverse, models/detector/yolo_ssod.py:158-172). */
 #define ETB_PACK_CHUNK 4096
 typedef struct EtbPackDesc {
   const float* w;   /* [Cout,Cin,k,k] fp32 */
@@ -365,9 +352,8 @@ typedef struct EtbFoldDesc {
   int32_t C;
   float eps;
 } EtbFoldDesc;
+/* eval-mode BatchNorm folded to per-channel scale/bias: scale = g/sqrt(var+eps), bias = b - mean*scale */
 int etb_fold_bn_multi(const EtbFoldDesc* descs_dev, int32_t n, void* stream);
-/* stem weight [Cout,3,6,6] fp32 -> [Cout][128] bf16 in the etb_stem_im2col K order */
-int etb_pack_stem_weight(const float* w_oihw, void* w_bf16, int32_t Cout, void* stream);
 
 /* ---- the last library ops of the student's step (csrc/tail.cu) ----------------------------------------------------------
  * Detect backward layout: the fused loss hands back d(loss)/d(logits) as fp32 [N,na,H,W,no] (the train layout of
@@ -400,9 +386,11 @@ typedef struct EtbFocalParams {
 int64_t etb_domain_focal_workspace_bytes(void);
 int etb_domain_focal_fwd(const EtbFocalParams* fp, float* out, void* workspace, int64_t workspace_bytes, void* stream);
 int etb_domain_focal_bwd(const EtbFocalParams* fp, const float* gout, void* stream);
-/* stem im2col straight from the loaders' batch (trainer/ssod_trainer.py:694-696 `imgs.to(device).float() / 255`): x is
- * [N,3,H,W] uint8 (is_u8) or fp32; value = x / div (IEEE division) rounded to bf16; the N images go to image slots
- * [img_offset, img_offset+N) of the im2col buffer y [*,H/2,W/2,128] -- torch.cat((imgs, unlabeled_imgs)) without the copy. */
+/* stem im2col straight from the loaders' batch (trainer/ssod_trainer.py:694-696 `imgs.to(device).float() / 255` fused with
+ * the 6x6 s2 p2 stem patch gather of models/backbone/yolov5_backbone.py:56): x is [N,3,H,W] uint8 (is_u8, div 255) or fp32
+ * (div 1 for already scaled input); value = x / div (IEEE division) rounded to bf16 at K index (c*6+kh)*6+kw (the OIHW
+ * weight row order) for K < 108, zeros above; the N images go to image slots [img_offset, img_offset+N) of the im2col
+ * buffer y [*,H/2,W/2,128] -- torch.cat((imgs, unlabeled_imgs)) without the copy. */
 int etb_stem_im2col_into(const void* x, int32_t is_u8, void* y_bf16, int32_t N, int32_t H, int32_t W, int32_t img_offset,
                          float div, void* stream);
 

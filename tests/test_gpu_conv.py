@@ -1,6 +1,5 @@
 """GPU (H100): the wgmma implicit-GEMM convolution and the trunk helpers against a plain PyTorch fp32 reference
 of the same op on bf16-rounded operands (floating-point kernel => torch reference, tolerance = bf16 output rounding)."""
-import numpy as np
 import pytest
 import torch
 import torch.nn.functional as F
@@ -113,9 +112,9 @@ def test_stem_im2col_conv():
     from efficientteacher_b200 import convops as co
     x = torch.rand((2, 3, 64, 64), generator=torch.Generator().manual_seed(9)).to(DEV) * 255.0
     w = _rand((64, 3, 6, 6), 10, scale=108 ** -0.5)
-    col = co.stem_im2col(x, mul=1.0 / 255.0)
+    col = co.stem_im2col_parts([x], 255.0)
     y = co.conv_fwd(col, co.pack_stem_weight(w), 128, 64, 1, 1, 0, None, None, act="silu")
-    ref = F.silu(F.conv2d(_bf(x * np.float32(1.0 / 255.0)), _bf(w), None, 2, 2))
+    ref = F.silu(F.conv2d(_bf(x / 255), _bf(w), None, 2, 2))
     _check(co.to_nchw_f32(y), ref)
 
 
@@ -270,7 +269,7 @@ def test_stem_wgrad():
     from efficientteacher_b200 import convops as co
     x = torch.rand((2, 3, 64, 64), generator=torch.Generator().manual_seed(41)).to(DEV)
     dy = _rand((2, 64, 32, 32), 42, scale=0.1)
-    col = co.stem_im2col(x, 1.0)
+    col = co.stem_im2col_parts([x])
     dw = co.conv_wgrad(col, co.to_nhwc_bf16(dy), 128, 64, 1, 1, 0, stem=True)
     ref = torch.nn.grad.conv2d_weight(_bf(x), (64, 3, 6, 6), _bf(dy), stride=2, padding=2)
     err = (dw - ref).abs().max().item()

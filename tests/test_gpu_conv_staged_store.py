@@ -73,7 +73,7 @@ def test_staged_store_equals_direct_store(case):
 def test_stem_staged_store():
     from efficientteacher_b200 import convops as co
     x = torch.rand((2, 3, 64, 96), generator=torch.Generator().manual_seed(9)).to(DEV) * 255.0
-    col = co.stem_im2col(x, mul=1.0 / 255.0)
+    col = co.stem_im2col_parts([x], 255.0)
     wp = co.pack_stem_weight(_rand((64, 3, 6, 6), 10, scale=108 ** -0.5))
     y = co.conv_fwd(col, wp, 128, 64, 1, 1, 0, None, None, act=None)
     assert torch.equal(y, co.conv_fwd(col, wp, 128, 64, 1, 1, 0, torch.ones(64, device=DEV), None, act=None))

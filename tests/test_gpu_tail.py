@@ -94,7 +94,7 @@ def test_stem_im2col_uint8_parts_equal_float_path():
     a = torch.from_numpy(r.randint(0, 256, (2, 3, 64, 96), dtype=np.uint8)).to(DEV)
     b = torch.from_numpy(r.randint(0, 256, (3, 3, 64, 96), dtype=np.uint8)).to(DEV)
     got = co.stem_im2col_parts([a, b], 255.0)
-    want = co.stem_im2col(torch.cat([a, b], 0).float() / 255.0, 1.0)       # trainer/ssod_trainer.py:694-696 then torch.cat (:620)
+    want = co.stem_im2col_parts([torch.cat([a, b], 0).float() / 255.0], 1.0)   # trainer/ssod_trainer.py:694-696 then torch.cat (:620)
     assert torch.equal(got, want)
     got_f = co.stem_im2col_parts([a.float() / 255.0, b.float() / 255.0], 1.0)
     assert torch.equal(got_f, want)

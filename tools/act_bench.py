@@ -44,7 +44,7 @@ def bn_kernels(dev):
         p = [_lib.ptr(t) for t in (y, da, stats[0], stats[1], stats[2], stats[3], out, part, sums)]
         for act in ACTS:
             a, s = co.ACT[act], _lib.stream_ptr()
-            t = {"apply": timeit(lambda: lib.etb_bn_act_apply(p[0], p[2], p[3], p[6], M, C_, C_, C_, a, s)),
+            t = {"apply": timeit(lambda: lib.etb_bn_act_apply_res(p[0], p[2], p[3], None, p[6], M, C_, C_, 0, C_, a, s)),
                  "bwd_reduce": timeit(lambda: lib.etb_bn_act_bwd_reduce(p[1], p[0], p[2], p[3], p[4], p[5], M, C_, C_, C_, a, p[7], rows1, s)),
                  "bwd_apply": timeit(lambda: lib.etb_bn_act_bwd_apply(p[1], p[0], p[2], p[3], p[4], p[5], p[8], M, C_, C_, C_, C_, a, p[6], s))}
             rows.append(dict(N=N, H=H, C=C_, act=act, **{k + "_us": round(v * 1e3, 2) for k, v in t.items()}))

@@ -32,7 +32,7 @@ def main():
         nb = M * C_ * 2
         r = {}
         r["stats(1R)"] = (timeit(lambda: lib.etb_bn_stats(_lib.ptr(y), M, C_, C_, _lib.ptr(part), rows0, _lib.stream_ptr())), 1)
-        r["apply(1R1W)"] = (timeit(lambda: lib.etb_bn_act_apply(_lib.ptr(y), _lib.ptr(stats[0]), _lib.ptr(stats[1]), _lib.ptr(out), M, C_, C_, C_, 1, _lib.stream_ptr())), 2)
+        r["apply(1R1W)"] = (timeit(lambda: lib.etb_bn_act_apply_res(_lib.ptr(y), _lib.ptr(stats[0]), _lib.ptr(stats[1]), None, _lib.ptr(out), M, C_, C_, 0, C_, 1, _lib.stream_ptr())), 2)
         r["bwd_reduce(2R)"] = (timeit(lambda: lib.etb_bn_act_bwd_reduce(_lib.ptr(da), _lib.ptr(y), _lib.ptr(stats[0]), _lib.ptr(stats[1]), _lib.ptr(stats[2]), _lib.ptr(stats[3]), M, C_, C_, C_, 1, _lib.ptr(part), rows1, _lib.stream_ptr())), 2)
         r["bwd_apply(2R1W)"] = (timeit(lambda: lib.etb_bn_act_bwd_apply(_lib.ptr(da), _lib.ptr(y), _lib.ptr(stats[0]), _lib.ptr(stats[1]), _lib.ptr(stats[2]), _lib.ptr(stats[3]), _lib.ptr(sums), M, C_, C_, C_, C_, 1, _lib.ptr(out), _lib.stream_ptr())), 3)
         print("M=%8d C=%4d (%6.1f MB/pass): " % (M, C_, nb / 1e6) + "  ".join("%s %6.1fus %4.0fGB/s(%.2f)" % (k, ms * 1e3, p * nb / ms / 1e6, p * nb / ms / 1e6 / pk) for k, (ms, p) in r.items()), flush=True)

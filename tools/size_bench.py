@@ -177,7 +177,7 @@ def bn_kernels(dev):
             p = [_lib.ptr(t) for t in (y, da, stats[0], stats[1], stats[2], stats[3], out, part1, sums, part0)]
             a, s = co.ACT["silu"], _lib.stream_ptr()
             kern = {"stats": (lambda: lib.etb_bn_stats(p[0], M, C_, C_, p[9], rows0, s), 2),
-                    "apply": (lambda: lib.etb_bn_act_apply(p[0], p[2], p[3], p[6], M, C_, C_, C_, a, s), 4),
+                    "apply": (lambda: lib.etb_bn_act_apply_res(p[0], p[2], p[3], None, p[6], M, C_, C_, 0, C_, a, s), 4),
                     "bwd_reduce": (lambda: lib.etb_bn_act_bwd_reduce(p[1], p[0], p[2], p[3], p[4], p[5], M, C_, C_, C_, a, p[7], rows1, s), 4),
                     "bwd_apply": (lambda: lib.etb_bn_act_bwd_apply(p[1], p[0], p[2], p[3], p[4], p[5], p[8], M, C_, C_, C_, C_, a, p[6], s), 6)}
             for name, (fn, bytes_per_elem) in kern.items():
