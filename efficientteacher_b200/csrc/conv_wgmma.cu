@@ -16,7 +16,7 @@
 //     each own 64 of the 128 pixel rows and issue wgmma.m64nBNk16 x4 per stage; the fp32 accumulator lives in their
 //     registers, and the epilogue (folded BN scale/bias -> SiLU -> +residual -> bf16 NHWC store at a channel offset of a
 //     wider buffer, so torch.cat is free) runs straight from those registers; the raw-output epilogue (EPI 0) stages the
-//     tile through shared memory first and stores whole pixel rows.
+//     tile in shared memory as bf16 and the producer warpgroup's second warp stores it by TMA (conv_store_warp).
 //   * every mbarrier wait is bounded (trap after ~2 s) so a descriptor bug cannot hang the GPU.
 #include "common.cuh"
 #include <cuda.h>
@@ -174,19 +174,22 @@ struct ConvKArgs {
   float* y_f32;
 };
 
-// EPI 0 stages each consumer warpgroup's fp32 accumulator through shared memory, half of its columns at a time
-// (64 rows x BN/2 fp32: 16 KB at BN = 128), so the global store goes out in 16 B vectors along the pixel rows.
+// EPI 0 stages the whole 128 x BN output tile as bf16 in the shared-memory image of the output tensor map's box
+// {64 ch, TW, TH, 1} under the 128 B swizzle: one 128-row x 128 B region per 64 channels (16 KB, 1024 B aligned), tile row
+// r = th*TW + tw, 16 B chunk q of row r at q ^ (r % 8).  32 KB at BN = 128, 16 KB at BN = 64.
 template <int BN, int EPI>
 struct ConvSmem {
   static constexpr int A_BYTES = CONV_BLOCK_M * 128;
   static constexpr int B_BYTES = BN * 128;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int STAGES = CONV_SMEM_STAGES_BYTES / STAGE_BYTES;   // 6 (BN = 128) or 8 (BN = 64)
-  static constexpr int OUT_BYTES = EPI == 0 ? 64 * (BN / 2) * 4 : 0;   // per consumer warpgroup
+  static constexpr int OUT_REGION = CONV_BLOCK_M * 128;                 // one 64-channel region of the staged tile
+  static constexpr int OUT_BYTES = EPI == 0 ? (BN / 64) * OUT_REGION : 0;
   static constexpr int OUT_OFF = STAGES * STAGE_BYTES;
-  static constexpr int BAR_OFF = OUT_OFF + 2 * OUT_BYTES;
+  static constexpr int BAR_OFF = OUT_OFF + OUT_BYTES;
   static constexpr int TOTAL = BAR_OFF + 256 + 1024;        // + barriers + slack for the 1024 B alignment
   static_assert(TOTAL <= 227 * 1024, "shared memory per block");
+  static_assert(OUT_OFF % 1024 == 0, "128 B swizzle atoms of the staged tile");
 };
 
 __device__ __forceinline__ float conv_act(float x, int act) {
@@ -197,8 +200,8 @@ __device__ __forceinline__ float conv_act(float x, int act) {
 
 // Epilogue of one consumer warpgroup's 64 x BN accumulator, straight from the wgmma fragment (see wgmma_m64n*k16): this
 // thread owns pixel rows r0 and r0+8 and, per 8-column block j, the channel pair 8j + 2*(lane%4) + {0,1}.  EPI selects the
-// fused tail at compile time so every register array is statically indexed (EPI 0 is conv_epilogue_staged below):
-//   EPI 0: raw bf16 store (+= existing when a.accumulate)       -- dgrad, training forward (conv_epilogue_staged)
+// fused tail at compile time so every register array is statically indexed (EPI 0 is conv_epilogue_stage below):
+//   EPI 0: raw bf16 store (+= existing when a.accumulate)       -- dgrad, training forward (conv_epilogue_stage)
 //   EPI 1: v*scale+bias (folded BN) -> SiLU/ReLU -> (+residual) -- teacher forward
 //   EPI 2: +bias, fp32 scatter into the Detect layout           -- head
 //   EPI 3: EPI 1 with Hardswish                                 -- teacher forward of Hardswish layers
@@ -254,102 +257,108 @@ __device__ __forceinline__ bool conv_out_pixel(const ConvKArgs& a, int img, int 
   return (row < a.TW * a.TH) && (oh < a.Ho) && (ow < a.Wo);
 }
 
-__device__ __forceinline__ void bar_sync_named(int id, int nthreads) {
-  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
-}
-__device__ __forceinline__ void st_shared_f2(uint32_t addr, float x, float y) {
-  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(x), "f"(y) : "memory");
-}
-__device__ __forceinline__ float4 ld_shared_f4(uint32_t addr) {
-  float4 v;
-  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr) : "memory");
+__device__ __forceinline__ uint32_t ld_shared_u32(uint32_t addr) {
+  uint32_t v;
+  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr) : "memory");
   return v;
 }
+__device__ __forceinline__ void st_shared_u32(uint32_t addr, uint32_t v) {
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+}
+// generic-proxy writes of shared memory -> visible to the TMA (async proxy) store that reads them
+__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+__device__ __forceinline__ void tma_store_4d(const CUtensorMap* map, const void* src, int c0, int c1, int c2, int c3) {
+  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
+               ::"l"((uint64_t)map), "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+__device__ __forceinline__ void bulk_wait_read_all() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
-// EPI 0: the warpgroup's 64 x BN accumulator goes out through its staging area `stg` (64 rows x BN/2 fp32) in two column
-// halves.  Each half: fragment -> stg (8 B stores), named barrier, then every thread takes 8 consecutive channels of one
-// row (two 16 B loads), adds the existing output when a.accumulate, rounds once to bf16 and stores 16 B, so a warp writes
-// whole 128-256 B runs of pixel rows instead of 8 rows x 16 B.  The values are those of a direct store from the fragment.
-// stg rows are 16 B chunks; chunk q of row r sits at q ^ 2*(r%4): the fragment stores (4 rows x 4 lanes per half-warp)
-// and the read-back (8 lanes of one 16 B phase take chunks 2g + h, h = bit 2 of the lane) are both free of bank conflicts.
+// EPI 0, consumer side: this thread's fragment (rows r and r+8, channel pair 8j + 2*(lane%4) per 8-column block j; see
+// wgmma_m64n*k16) goes into the staged tile `stg` (ConvSmem layout) as bf16 pairs.  With a.accumulate the staged tile
+// already holds the tile's existing output (TMA-loaded by the store warp) and each pair is read, added in fp32 and rounded
+// once, which is the value of old + acc rounded once.  Regions that lie wholly past Cout are neither loaded nor stored.
+// A warp's 4 B accesses cover 8 consecutive rows x 4 lanes: the swizzle puts the 8 rows in 8 distinct 16 B chunks, so
+// they are free of bank conflicts.
 template <int BN>
-__device__ __forceinline__ void conv_epilogue_staged(const ConvKArgs& a, const float* d, int n0, int img, int th_i, int tw_i, int cw,
-                                                     uint32_t stg) {
-  constexpr int HALF = BN / 2;               // columns per half
-  constexpr int PITCH = HALF * 4;            // bytes per staged row
-  constexpr int GPR = HALF / 8;              // 8-channel groups per row: 8 (BN = 128) or 4 (BN = 64)
-  constexpr int RPI = 128 / GPR;             // rows read back per pass of the warpgroup
-  const int t = threadIdx.x & 127, lane = threadIdx.x & 31;
-  const int r_frag = 16 * (t >> 5) + (lane >> 2);
-  const int g = t % GPR, h = (lane >> 2) & 1;
+__device__ __forceinline__ void conv_epilogue_stage(const ConvKArgs& a, const float* d, int n0, int row, int lane, uint32_t stg) {
+  const uint32_t base = stg + row * 128 + 4 * (lane & 3);
+  const int sw = row & 7;                      // also the swizzle of row + 8
 #pragma unroll
-  for (int hf = 0; hf < 2; ++hf) {
-    if (n0 + hf * HALF >= a.Cout) break;     // uniform: the whole half lies beyond Cout
+  for (int j = 0; j < BN / 8; ++j) {
+    if ((j & 7) == 0 && n0 + 8 * j >= a.Cout) break;     // uniform: the region lies beyond Cout
 #pragma unroll
-    for (int jj = 0; jj < HALF / 8; ++jj) {
-      const int j = hf * (HALF / 8) + jj;
-#pragma unroll
-      for (int i = 0; i < 2; ++i) {
-        const int r = r_frag + 8 * i;
-        const int q = 2 * jj + ((lane & 3) >> 1);
-        st_shared_f2(stg + r * PITCH + ((q ^ ((r & 3) << 1)) << 4) + ((lane & 1) << 3), d[j * 4 + i * 2], d[j * 4 + i * 2 + 1]);
+    for (int i = 0; i < 2; ++i) {
+      const uint32_t addr = base + (j >> 3) * ConvSmem<BN, 0>::OUT_REGION + i * 8 * 128 + (((j & 7) ^ sw) << 4);
+      float v0 = d[j * 4 + i * 2], v1 = d[j * 4 + i * 2 + 1];
+      if (a.accumulate) {
+        const uint32_t old = ld_shared_u32(addr);
+        const float2 f = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&old));
+        v0 += f.x;
+        v1 += f.y;
       }
+      const __nv_bfloat162 o = __floats2bfloat162_rn(v0, v1);
+      st_shared_u32(addr, *reinterpret_cast<const uint32_t*>(&o));
     }
-    bar_sync_named(1 + cw, 128);
-    const int gc = n0 + hf * HALF + 8 * g;
-#pragma unroll 1
-    for (int it = 0; it < 64 / RPI; ++it) {
-      const int r = it * RPI + t / GPR;
-      const int sw = (r & 3) << 1;
-      const float4 c0 = ld_shared_f4(stg + r * PITCH + (((2 * g + h) ^ sw) << 4));
-      const float4 c1 = ld_shared_f4(stg + r * PITCH + (((2 * g + 1 - h) ^ sw) << 4));
-      const float4 lo = h ? c1 : c0, hi = h ? c0 : c1;
-      float v[8] = {lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w};
-      size_t pix;
-      if (!conv_out_pixel(a, img, th_i, tw_i, 64 * cw + r, &pix) || gc >= a.Cout) continue;
-      __nv_bfloat16* yp = a.y + pix * a.y_cstride + a.y_coffset + gc;
-      if (gc + 8 <= a.Cout) {
-        if (a.accumulate) {
-          const uint4 pv = *reinterpret_cast<const uint4*>(yp);
-          const __nv_bfloat162* p2 = reinterpret_cast<const __nv_bfloat162*>(&pv);
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            const float2 f = __bfloat1622float2(p2[k]);
-            v[2 * k] += f.x;
-            v[2 * k + 1] += f.y;
-          }
-        }
-        uint4 o;
-        __nv_bfloat162* o2 = reinterpret_cast<__nv_bfloat162*>(&o);
-#pragma unroll
-        for (int k = 0; k < 4; ++k) o2[k] = __floats2bfloat162_rn(v[2 * k], v[2 * k + 1]);
-        *reinterpret_cast<uint4*>(yp) = o;
-      } else {                                 // Cout % 8 != 0: the last group of channels is partial
-#pragma unroll
-        for (int k = 0; k < 8; ++k) {
-          if (gc + k >= a.Cout) break;
-          float x = v[k];
-          if (a.accumulate) x += __bfloat162float(yp[k]);
-          yp[k] = __float2bfloat16(x);
-        }
-      }
-    }
-    bar_sync_named(1 + cw, 128);             // stg is rewritten by the next half / tile
   }
+}
+
+// EPI 0, store side: warp 1 walks the CTA's tiles in the consumers' order, one lane issuing (bulk groups belong to the
+// issuing thread).  Per tile:
+//   a.accumulate: TMA-load the tile's existing output into the staged tile (free: first tile, or the previous tile's
+//     stores have finished reading it) -> acc_full; this runs while the consumers are in the tile's K loop;
+//   wait stg_full (all 256 consumer threads have written the tile and fenced) -> one bulk tensor store per 64-channel
+//   region inside Cout -> wait until the stores have read shared memory -> stg_empty.
+// The consumers wait for stg_empty only before they next write the tile, a whole K loop later.  TMA clips every box
+// at Cout, at the edges of the output lattice and at the last pixel, so nothing outside the output is written.
+template <int BN>
+__device__ __forceinline__ void conv_store_warp(const CUtensorMap* mapY, const ConvKArgs& a, uint8_t* stg, uint64_t* stg_full,
+                                                uint64_t* stg_empty, uint64_t* acc_full, int n_tiles, int total_tiles) {
+  const bool leader = (threadIdx.x & 31) == 0;
+  uint32_t ph = 0;
+  for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ph ^= 1u) {
+    const int n0 = (tile % n_tiles) * BN;
+    int t = tile / n_tiles;
+    const int tw_i = t % a.tiles_w; t /= a.tiles_w;
+    const int th_i = t % a.tiles_h; t /= a.tiles_h;
+    const int c1 = tw_i * a.TW, c2 = th_i * a.TH, img = t;
+    const int nreg = min(BN / 64, (a.Cout - n0 + 63) / 64);
+    if (a.accumulate && leader) {
+      mbar_expect_tx(acc_full, (uint32_t)(nreg * a.TW * a.TH * 128));
+      for (int r = 0; r < nreg; ++r) tma_load_4d(mapY, acc_full, stg + r * ConvSmem<BN, 0>::OUT_REGION, n0 + 64 * r, c1, c2, img);
+    }
+    mbar_wait(stg_full, ph);
+    if (leader) {
+      for (int r = 0; r < nreg; ++r) tma_store_4d(mapY, stg + r * ConvSmem<BN, 0>::OUT_REGION, n0 + 64 * r, c1, c2, img);
+      bulk_commit();
+      bulk_wait_read_all();
+      mbar_arrive(stg_empty);
+    }
+    __syncwarp();
+  }
+  if (leader) bulk_wait_all();                 // the stores are complete before the CTA exits
 }
 
 // Persistent: gridDim.x CTAs walk the tile list (tile = blockIdx.x + i*gridDim.x; N tile fastest so the CTAs running
 // concurrently share A tiles in L2).  The smem ring runs across tile boundaries, so the producer streams the operands of
-// tile i+1 while the consumers run the epilogue of tile i.
+// tile i+1 while the consumers run the epilogue of tile i.  EPI 0 hands each tile to the store warp (conv_store_warp) through
+// the staged tile in shared memory and goes straight on to the next tile's K loop; mapY is its output map (unused by
+// EPI 1-3, which store from registers).
 template <int BN, int EPI>
 __global__ void __launch_bounds__(CONV_THREADS, 1)
-conv_fwd_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB, const ConvKArgs a) {
+conv_fwd_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB,
+                const __grid_constant__ CUtensorMap mapY, const ConvKArgs a) {
   using L = ConvSmem<BN, EPI>;
   constexpr int STAGES = L::STAGES;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   uint64_t* full = (uint64_t*)(smem + L::BAR_OFF);
   uint64_t* empty = full + STAGES;
+  uint64_t* stg_full = empty + STAGES;     // EPI 0: consumers -> store warp, the staged tile is written
+  uint64_t* stg_empty = stg_full + 1;      //        store warp -> consumers, the stores have read it
+  uint64_t* acc_full = stg_full + 2;       //        store warp -> consumers, the existing output is loaded (a.accumulate)
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int wg = warp >> 2;
@@ -362,11 +371,21 @@ conv_fwd_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
     tma_prefetch_desc(&mapA);
     tma_prefetch_desc(&mapB);
     for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }   // 8 consumer warps release a stage
+    if (EPI == 0) {
+      tma_prefetch_desc(&mapY);
+      mbar_init(stg_full, 256);
+      mbar_init(stg_empty, 1);
+      mbar_init(acc_full, 1);
+    }
     fence_barrier_init();
   }
   __syncthreads();
 
   if (wg == 0) {
+    if (EPI == 0 && warp == 1) {
+      conv_store_warp<BN>(&mapY, a, smem + L::OUT_OFF, stg_full, stg_empty, acc_full, n_tiles, total_tiles);
+      return;
+    }
     if (warp != 0) return;
     // ===== TMA producer: the whole warp runs the loop (uniform), one elected lane issues =====
     const uint32_t a_bytes = (uint32_t)(a.TW * a.TH * 128);
@@ -405,6 +424,7 @@ conv_fwd_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
   float d[BN / 2];
   int s = 0;
   uint32_t ph = 0;
+  uint32_t tph = 0;                // EPI 0: parity of the staged-tile barriers, one phase per tile
   for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
     int prev = -1;
     for (int ki = 0; ki < kiters; ++ki) {
@@ -425,13 +445,18 @@ conv_fwd_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
     acc_fence<BN / 2>(d);
     if (lane == 0) mbar_arrive(&empty[prev]);
     const int n0 = (tile % n_tiles) * BN;
-    int t = tile / n_tiles;
-    const int tw_i = t % a.tiles_w; t /= a.tiles_w;
-    const int th_i = t % a.tiles_h; t /= a.tiles_h;
-    const int img = t;
     if constexpr (EPI == 0) {
-      conv_epilogue_staged<BN>(a, d, n0, img, th_i, tw_i, cw, smem_u32(smem + L::OUT_OFF + cw * L::OUT_BYTES));
+      mbar_wait(stg_empty, tph ^ 1u);          // the previous tile's stores have read the staged tile
+      if (a.accumulate) mbar_wait(acc_full, tph);
+      conv_epilogue_stage<BN>(a, d, n0, rbase, lane, smem_u32(smem + L::OUT_OFF));
+      fence_proxy_async_smem();
+      mbar_arrive(stg_full);
+      tph ^= 1u;
     } else {
+      int t = tile / n_tiles;
+      const int tw_i = t % a.tiles_w; t /= a.tiles_w;
+      const int th_i = t % a.tiles_h; t /= a.tiles_h;
+      const int img = t;
       bool row_ok[2];
       size_t pix[2];
 #pragma unroll
@@ -472,23 +497,36 @@ static void pick_tile(int Wo, int Ho, int* TW, int* TH) {
 }
 
 template <int BN, int EPI>
-static int launch_conv_e(const CUtensorMap& mA, const CUtensorMap& mB, const ConvKArgs& ka, dim3 grid, cudaStream_t st) {
+static int launch_conv_e(const CUtensorMap& mA, const CUtensorMap& mB, const CUtensorMap& mY, const ConvKArgs& ka, dim3 grid,
+                         cudaStream_t st) {
   using L = ConvSmem<BN, EPI>;
   static bool attr_set = false;
   if (!attr_set) {
     ETB_CHECK_CUDA(cudaFuncSetAttribute(conv_fwd_kernel<BN, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::TOTAL));
     attr_set = true;
   }
-  etb_launch(conv_fwd_kernel<BN, EPI>, dim3(grid), dim3(CONV_THREADS), L::TOTAL, st, mA, mB, ka);
+  etb_launch(conv_fwd_kernel<BN, EPI>, dim3(grid), dim3(CONV_THREADS), L::TOTAL, st, mA, mB, mY, ka);
   ETB_CHECK_LAUNCH();
   return ETB_OK;
 }
+// The epilogue instance a launch runs (see conv_epilogue).  EPI 0's TMA store writes whole 16 B channel groups (the box
+// is not clipped inside one), so a raw output whose Cout is not a multiple of 8 goes through EPI 1 with scale 1, bias 0
+// and no activation, which stores the same values from registers channel by channel (no trunk width needs it).
+static int conv_epi(const ConvKArgs& ka) {
+  if (ka.out_mode == 1) return 2;
+  if (ka.act == 4) return 3;
+  if (ka.scale || ka.bias || ka.act || ka.residual || ka.Cout % 8 != 0) return 1;
+  return 0;
+}
 template <int BN>
-static int launch_conv(const CUtensorMap& mA, const CUtensorMap& mB, const ConvKArgs& ka, dim3 grid, cudaStream_t st) {
-  if (ka.out_mode == 1) return launch_conv_e<BN, 2>(mA, mB, ka, grid, st);
-  if (ka.act == 4) return launch_conv_e<BN, 3>(mA, mB, ka, grid, st);
-  if (ka.scale || ka.bias || ka.act || ka.residual) return launch_conv_e<BN, 1>(mA, mB, ka, grid, st);
-  return launch_conv_e<BN, 0>(mA, mB, ka, grid, st);
+static int launch_conv(const CUtensorMap& mA, const CUtensorMap& mB, const CUtensorMap& mY, const ConvKArgs& ka, dim3 grid,
+                       cudaStream_t st) {
+  switch (conv_epi(ka)) {
+    case 2: return launch_conv_e<BN, 2>(mA, mB, mY, ka, grid, st);
+    case 3: return launch_conv_e<BN, 3>(mA, mB, mY, ka, grid, st);
+    case 1: return launch_conv_e<BN, 1>(mA, mB, mY, ka, grid, st);
+    default: return launch_conv_e<BN, 0>(mA, mB, mY, ka, grid, st);
+  }
 }
 
 // One implicit-GEMM launch: D[pixels, rows_B] = sum_taps A(shifted) * B^T.  `ka` carries the epilogue.
@@ -564,10 +602,31 @@ static int launch_gemm(const GemmGeom& g, ConvKArgs ka, cudaStream_t st) {
   ka.kblocks = aCp / CONV_BLOCK_K;
   ka.Cout = g.b_rows;
   ka.nimg = nimg;
+  // EPI 0 output map: the Ho x Wo output lattice (pixel (oh,ow) at (oh*out_os+out_ph, ow*out_os+out_pw) of the out_H x
+  // out_W plane) inside the channel slice [y_coffset, +Cout) of y, box = one 64-channel region of the staged tile.  The
+  // flat tiling is the lattice 1 x npix.  All strides are multiples of 16 B (y_cstride % 8 == 0).
+  CUtensorMap mY;
+  memset(&mY, 0, sizeof(mY));
+  ETB_CHECK_ARG(!ka.accumulate || conv_epi(ka) == 0);   // only EPI 0 accumulates
+  if (conv_epi(ka) == 0) {
+    const cuuint64_t cs = (cuuint64_t)ka.y_cstride * 2;
+    cuuint64_t ydim[4] = {(cuuint64_t)ka.Cout, (cuuint64_t)ka.Wo, (cuuint64_t)ka.Ho, (cuuint64_t)nimg};
+    cuuint64_t ystr[3] = {cs * ka.out_os, cs * ka.out_os * ka.out_W, cs * ka.out_W * ka.out_H};
+    cuuint32_t ybox[4] = {64, (cuuint32_t)ka.TW, (cuuint32_t)ka.TH, 1};
+    cuuint32_t yestr[4] = {1, 1, 1, 1};
+    __nv_bfloat16* ybase = ka.y + ((size_t)ka.out_ph * ka.out_W + ka.out_pw) * ka.y_cstride + ka.y_coffset;
+    ETB_CHECK_ARG((((uintptr_t)ybase) & 15) == 0);
+    r = enc(&mY, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, ybase, ydim, ystr, ybox, yestr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+            CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) {
+      etb_set_error("cuTensorMapEncodeTiled(Y) failed: %d", (int)r);
+      return ETB_ERR_CUDA;
+    }
+  }
   const long total_tiles = (long)ka.tiles_w * ka.tiles_h * nimg * ((g.b_rows + BN - 1) / BN);
   const long resident = (long)etb_num_sms();   // persistent: one CTA per SM (the operand ring takes 192 KB of shared memory)
   dim3 grid((unsigned)(total_tiles < resident ? total_tiles : resident), 1);
-  return BN == 128 ? launch_conv<128>(mA, mB, ka, grid, st) : launch_conv<64>(mA, mB, ka, grid, st);
+  return BN == 128 ? launch_conv<128>(mA, mB, mY, ka, grid, st) : launch_conv<64>(mA, mB, mY, ka, grid, st);
 }
 
 extern "C" int etb_conv_fwd(const void* x_bf16, const void* w_bf16, const float* scale, const float* bias,

@@ -1,5 +1,7 @@
-"""Per-layer-shape timing of the wgmma conv kernels (fwd / dgrad / wgrad) on the YOLOv5l@640 shapes, CUDA events,
-L2 flushed between iterations.  python tools/conv_bench.py [--batch 16] [--out bench_out/conv_bench.json]"""
+"""Per-layer-shape timing of the wgmma conv kernels on the YOLOv5l@640 shapes, CUDA events, L2 flushed between iterations.
+Modes: fwd (folded BN + SiLU), raw (raw output: the student's training forward), dgrad, dgrad_acc (dgrad added into the
+existing input gradient: gradient fan-in), wgrad.
+  python tools/conv_bench.py [--batch 16] [--modes fwd,dgrad,wgrad] [--out bench_out/conv_bench.json]"""
 import argparse
 import json
 import os
@@ -113,6 +115,12 @@ def main():
             ms = timeit(lambda: co.conv_dgrad(dy, wd, N, H, H, Cin, Cout, k, s, p, out=dx))
             row["dgrad_us"], row["dgrad_tflops"] = ms * 1e3, flops / ms / 1e9
             tot["dgrad"][0] += ms * cnt; tot["dgrad"][1] += flops * cnt
+        if "dgrad_acc" in tot and Cout % 64 == 0:   # gradient fan-in: the dgrad is added into the existing input gradient
+            wd = co.pack_weight_dgrad(w, s, p)
+            dx = torch.zeros(N, H, H, Cin, dtype=torch.bfloat16, device=dev)
+            ms = timeit(lambda: co.conv_dgrad(dy, wd, N, H, H, Cin, Cout, k, s, p, out=dx, accumulate=True))
+            row["dgrad_acc_us"], row["dgrad_acc_tflops"] = ms * 1e3, flops / ms / 1e9
+            tot["dgrad_acc"][0] += ms * cnt; tot["dgrad_acc"][1] += flops * cnt
         if "wgrad" in tot:
             ms = timeit(lambda: co.conv_wgrad(x, dy, Cin, Cout, k, s, p))
             row["wgrad_us"], row["wgrad_tflops"] = ms * 1e3, flops / ms / 1e9
