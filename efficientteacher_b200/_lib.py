@@ -160,6 +160,10 @@ _SIGS = {
     "etb_tal_assign": (C.c_int, [vp, vp, vp, vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_float, C.c_float,
                                 C.c_float, vp, vp, vp, vp, vp, C.c_size_t, vp]),
     "etb_v8_decode": (C.c_int, [vp, vp, C.POINTER(EtbV8Levels), C.c_int32, C.c_int32, C.c_int32, C.c_float, vp, vp, vp, vp, vp]),
+    "etb_pl_quality_workspace_bytes": (C.c_size_t, []),
+    "etb_pl_quality": (C.c_int, [vp, vp, C.c_int32, vp, vp, C.c_int32, vp, vp, C.c_int32, vp, C.c_int32, C.c_int32, C.c_int32,
+                                 C.c_int32, vp, vp, vp, C.c_size_t, vp]),
+    "etb_meter_update": (C.c_int, [vp, C.c_int32, C.POINTER(vp), C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int32, vp]),
 }
 
 _lib = None

@@ -18,7 +18,7 @@ import importlib
 import inspect
 import sys
 
-from . import _lib, ema, labelmatch, loss, metrics, model, nms, pseudo_label, ssod_loss, assigner, tal
+from . import _lib, ema, labelmatch, loss, metrics, model, nms, pl_quality, pseudo_label, ssod_loss, assigner, tal
 from . import val as etb_val
 
 _lib.lib()  # fail loudly now if the kernels are not built
@@ -89,6 +89,8 @@ _PATCHES = [
     ("utils.metrics", "ap_per_class", _ap_per_class),
     ("val", "run", _val_run),
     ("utils.self_supervised_utils", "FairPseudoLabel", pseudo_label.FairPseudoLabel),
+    ("utils.self_supervised_utils", "check_pseudo_label_with_gt", pl_quality.check_pseudo_label_with_gt),   # ssod_trainer.py:46
+    ("utils.self_supervised_utils", "check_pseudo_label", pl_quality.check_pseudo_label),
     ("utils.labelmatch", "LabelMatch", labelmatch.LabelMatch),
     ("models.loss.loss", "ComputeLoss", loss.ComputeLoss),
     ("models.loss.ssod.ssod_loss", "ComputeStudentMatchLoss", ssod_loss.ComputeStudentMatchLoss),

@@ -33,7 +33,7 @@ def _ssod():
               pseudo_label_with_obj=True, pseudo_label_with_bbox=True, pseudo_label_with_cls=False, with_da_loss=False,
               da_loss_weights=0.01, epoch_adaptor=True, ema_rate=0.999, cosine_ema=True, imitate_teacher=False,
               focal_loss=0.0, pseudo_label_type='FairPseudoLabel', debug=False, fixed_accumulate=False,
-              extra_teachers=[], multi_step_lr=False, milestones=[10, 20])
+              extra_teachers=[], multi_step_lr=False, milestones=[10, 20], ssod_hyp=NS(with_gt=False))
 
 
 # (depth_multiple, width_multiple) of the reference's five YOLOv5 sizes (configs/sup/public/yolov5{n,s,m,l,x}_coco.yaml),

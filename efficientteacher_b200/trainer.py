@@ -28,6 +28,7 @@ from .loss import ComputeLoss
 from .model import Model, SupModel
 from .optim import FusedAdamW, FusedSGD
 from .parallel import GradArena
+from .pl_quality import HIT_KEYS, DeviceMetricMeter, PLQuality
 from .pseudo_label import FairPseudoLabel
 from .ssod_loss import ComputeStudentMatchLoss
 
@@ -75,6 +76,7 @@ class TrainerStep:
         self._arena = None
         self._bn_sync = None
         self.last = {}
+        self.meter = DeviceMetricMeter(device)     # trainer/trainer.py:370 (rank 0's MetricMeter; here every rank keeps one)
         self.profile = False     # record CUDA events at the phase boundaries of the eager step
         self.phase_events = []
         self._graph = None       # the step captured as CUDA graphs (see _graphed)
@@ -210,28 +212,40 @@ class TrainerStep:
     # ---- the labels of a captured step: a static buffer of capacity C and the count in a device int32 -----------------
     LABEL_CAPACITY = 64      # initial label capacity of a captured SSOD / supervised step; doubles when a batch has more labels
 
-    def _label_capacity(self, slot, targets, initial):
+    # The same scheme holds the SSOD step's unlabeled ground truth: buffer "ugt", count "nug", capacity "gcap".
+    def _label_capacity(self, slot, targets, initial, cap="cap"):
         """The label capacity of the graph in `slot` (`initial` before the first capture), doubled until the batch's
         labels fit.  It goes into the capture key, so only a batch with more labels than the capacity re-captures."""
-        cap = initial if getattr(self, slot) is None else getattr(self, slot)["cap"]
-        while cap < targets.shape[0]:
-            cap *= 2
-        return cap
+        c = initial if getattr(self, slot) is None else getattr(self, slot).get(cap, initial)
+        while c < targets.shape[0]:
+            c *= 2
+        return c
 
-    def _static_labels(self, g, cap, targets):
+    def _static_labels(self, g, cap, targets, buf="targets", count="nt", cap_key="cap"):
         """g["targets"] [cap, 6] fp32 and g["nt"] int32[1], filled from the capturing call.  The loss (ComputeLoss(...,
         n_dev)) and LabelMatch's histogram read only the first nt rows, so one graph serves every label count <= cap."""
         nt = int(targets.shape[0])
-        g.update(cap=cap, targets=torch.zeros((cap, 6), dtype=torch.float32, device=self.device),
-                 nt=torch.full((1,), nt, dtype=torch.int32, device=self.device))
-        g["targets"][:nt].copy_(targets)
+        g.update({cap_key: cap, buf: torch.zeros((cap, 6), dtype=torch.float32, device=self.device),
+                  count: torch.full((1,), nt, dtype=torch.int32, device=self.device)})
+        g[buf][:nt].copy_(targets)
 
-    def _stage_labels(self, g, targets):
+    def _stage_labels(self, g, targets, buf="targets", count="nt"):
         """one call's labels (CPU or CUDA) into the static buffers, stream-ordered, without a host sync"""
         nt = int(targets.shape[0])
-        g["targets"][:nt].copy_(targets, non_blocking=True)
+        g[buf][:nt].copy_(targets, non_blocking=True)
         # pageable source: the runtime stages these few bytes before returning, so the next step cannot overwrite them early
-        g["nt"].copy_(torch.tensor([nt], dtype=torch.int32))
+        g[count].copy_(torch.tensor([nt], dtype=torch.int32))
+
+    def _log(self, loss, items):
+        """trainer.py:434 / ssod_trainer.py:447,524: the meter takes ComputeLoss's box obj cls loss; self.last the detached
+        loss and items"""
+        self.meter.update(items)
+        self.last = dict(loss=loss.detach(), sup={k: v.detach() for k, v in items.items()})
+
+    def reset_meter(self):
+        """trainer/trainer.py:370 (before_epoch: a new MetricMeter): the meter's sums and counts start again from zero, in
+        place, so the captured steps keep updating it without a re-capture"""
+        self.meter.reset()
 
     # ---- the whole step as CUDA graphs ------------------------------------------------------------------------------
     def _graphed(self, slot, key, hooks, inputs, ni):
@@ -260,6 +274,7 @@ class TrainerStep:
             self.optimizer.refresh_hyper()
         self._bn_broadcast()
         g["graph"].replay()
+        self.last = g["last"]                # this iteration's loss items: the graph's static outputs, valid until the next replay
         if due:
             self._allreduce_grads()          # one all-reduce per optimizer step, between the two graphs (enqueued, no host sync)
             g["graph_b"].replay()
@@ -294,7 +309,7 @@ class TrainerStep:
             graph = torch.cuda.CUDAGraph()
             with torch.cuda.graph(graph):
                 g["loss"] = hooks.body(self, g)
-            g["graph"] = graph
+            g["graph"], g["last"] = graph, self.last
             gb = torch.cuda.CUDAGraph()
             with torch.cuda.graph(gb, pool=graph.pool()):
                 self.optimizer.step(zero_grad=True)
@@ -310,8 +325,8 @@ class TrainerStep:
     def _snapshot_training_state(self):
         """The warm-up steps before a capture really train: snapshot every piece of state they touch (weights, BN
         statistics, the EMA model(s), the optimizer state -- SGD momentum, or AdamW's moments and step count --, the
-        gradients accumulated towards the next optimizer step, the counters, lr / momentum) and return the function that
-        puts it back."""
+        gradients accumulated towards the next optimizer step, the training meter, the counters, lr / momentum) and return
+        the function that puts it back."""
         self._ensure_arena()
         emas = [e for e in (self.ema, self.semi_ema) if e is not None]
         opt_keys = ("momentum_buffer", "exp_avg", "exp_avg_sq")
@@ -321,6 +336,7 @@ class TrainerStep:
             tensors += [self.optimizer.state[p][k] for g_ in self.optimizer.param_groups for p in g_["params"]
                         for k in opt_keys if self.optimizer.state[p].get(k) is not None]
         tensors.append(self._arena.flat)     # gradients already accumulated towards the next optimizer step (accumulate > 1)
+        tensors.append(self.meter.state)
         snap = [t.clone() for t in tensors]
         saved = (self.last_opt_step, [e.updates for e in emas], self.accumulate,
                  [(x['lr'], x.get('momentum')) for x in self.optimizer.param_groups])
@@ -379,6 +395,7 @@ class SSODTrainerStep(TrainerStep):
         self._teacher_keep = None
         self._burn_graph = None     # captured burn-in step (train_without_unlabeled[_da]_graphed)
         self.burn_in_captures = 0   # how many times a burn-in step has been captured
+        self._plq = PLQuality(device)   # the pseudo-label statistics of the step (iouv = [0.5], ssod_trainer.py:662)
 
     # trainer/ssod_trainer.py:86-94: SSOD.multi_step_lr replaces the LambdaLR by MultiStepLR(milestones, gamma=0.1) on top
     # of it (the warm-up still interpolates towards initial_lr * lf(epoch)); the supervised step has no such switch
@@ -404,12 +421,28 @@ class SSODTrainerStep(TrainerStep):
         ps = [split_batch(p, n_img) for p in total_pred]
         return [a for a, _ in ps], [a for a, _ in fs], [b for _, b in ps], [b for _, b in fs]
 
-    # trainer/ssod_trainer.py:587-680 (logging / meters excluded: rank-0 host bookkeeping)
+    @property
+    def with_gt(self):
+        """SSOD.ssod_hyp.with_gt (configs/defaults.py:303, default False): score the pseudo labels against the unlabeled
+        images' ground truth (check_pseudo_label_with_gt) rather than by their reliable / uncertain split (check_pseudo_label)"""
+        return bool(getattr(getattr(self.cfg.SSOD, 'ssod_hyp', None), 'with_gt', False))
+
+    def _hit_rate(self, rows, n_dev, gt, m_dev):
+        """ssod_trainer.py:661-671: tp fp_cls fp_loc pse_num gt_num of this step's pseudo labels as device scalars (views of
+        the etb_pl_quality output), with the thresholds the unsupervised loss selects by, and batch_size // WORLD_SIZE"""
+        hi, lo = self.compute_un_sup_loss._thresholds(self.device)
+        vals = self._plq.run(rows.contiguous(), n_dev, hi, lo, gt if self.with_gt else None, m_dev,
+                             self.batch_size // self.WORLD_SIZE, self.with_gt)
+        return {k: vals[i, 0] for i, k in enumerate(HIT_KEYS)}
+
+    # trainer/ssod_trainer.py:587-680; the meter update of :653-672 on the device
     def train_instance(self, imgs, targets, unlabeled_imgs, unlabeled_imgs_ori, unlabeled_gt, unlabeled_M, ni,
-                       host_pseudo_labels=False, _stop_after_backward=False, _n_dev=None):
-        """_stop_after_backward: the body of the captured graph A (TrainerStep._graphed), which ends after the backward and
-        leaves LabelMatch's image counters to the replay wrapper.  _n_dev (int32[1] CUDA): targets is a padded label
-        buffer whose first _n_dev rows are the labels (ComputeLoss(..., n_dev), LabelMatch.update_device(..., n_dev))."""
+                       host_pseudo_labels=False, _stop_after_backward=False, _n_dev=None, _m_dev=None):
+        """unlabeled_gt [M,6] (img, cls, x, y, w, h normalised; None: no boxes) feeds the pseudo-label statistics when
+        with_gt.  _stop_after_backward: the body of the captured graph A (TrainerStep._graphed), which ends after the backward
+        and leaves LabelMatch's image counters to the replay wrapper.  _n_dev (int32[1] CUDA): targets is a padded label
+        buffer whose first _n_dev rows are the labels (ComputeLoss(..., n_dev), LabelMatch.update_device(..., n_dev));
+        _m_dev likewise for unlabeled_gt."""
         self._require_semi_ema()
         n_img = imgs.shape[0]
         self._mark("start")
@@ -469,39 +502,49 @@ class SSODTrainerStep(TrainerStep):
         if invalid_target_shape:
             un_sup_loss = torch.zeros(1, device=self.device)
             un_sup_loss_items = dict(ss_box=0, ss_obj=0, ss_cls=0)
+            hit_rate = dict(tp=0, fp_cls=0, fp_loc=0, pse_num=0, gt_num=0)     # no pseudo label created (:658-660)
         else:
             un_sup_loss, un_sup_loss_items = self.compute_un_sup_loss(un_sup_pred, unlabeled_targets, n_dev)
+            if self.with_gt and unlabeled_gt is not None and _m_dev is None:
+                unlabeled_gt = unlabeled_gt.to(self.device, torch.float32).reshape(-1, 6).contiguous()
+            hit_rate = self._hit_rate(unlabeled_targets, n_dev, unlabeled_gt, _m_dev)
         # DDP: loss*WORLD_SIZE then gradient mean == plain SUM all-reduce of per-rank gradients (no scaling here)
         loss = sup_loss + un_sup_loss * self.cfg.SSOD.teacher_loss_weight
         self._mark("losses")
+        # box obj cls loss ss_box ss_obj ss_cls tp fp_cls fp_loc pse_num gt_num, the reference's key order (:653-672)
+        self.meter.update({**sup_loss_items, **un_sup_loss_items, **hit_rate})
+        # logging values only -- detached, so that no reference to this step's autograd graph (and to the AccumulateGrad
+        # nodes of the parameters, which are tied to the stream they were created on) survives the step
+        det = lambda d: {k: (v.detach() if torch.is_tensor(v) else v) for k, v in d.items()}  # noqa: E731
+        self.last = dict(loss=loss.detach(), sup=det(sup_loss_items), unsup=det(un_sup_loss_items), hits=hit_rate)
         if _stop_after_backward:         # captured graph A ends here
             self._backward(loss)
             return loss.detach()
         self.update_optimizer(loss, ni)
         self._mark("optimizer_ema")
-        # logging values only -- detached, so that no reference to this step's autograd graph (and to the AccumulateGrad
-        # nodes of the parameters, which are tied to the stream they were created on) survives the step
-        det = lambda d: {k: (v.detach() if torch.is_tensor(v) else v) for k, v in d.items()}  # noqa: E731
-        self.last = dict(loss=loss.detach(), sup=det(sup_loss_items), unsup=det(un_sup_loss_items))
         return loss.detach()
 
     # ---- the whole step as CUDA graphs ------------------------------------------------------------------------------
-    def _ssod_static(self, key, imgs, targets, us, uw, Ms):
-        g = dict(imgs=imgs.clone(), us=us.clone(), uw=uw.clone(), Ms=Ms.to(self.device, torch.float64).clone())
-        self._static_labels(g, key[-1], targets)
+    def _ssod_static(self, key, imgs, targets, us, uw, Ms, ugt):
+        g = dict(imgs=imgs.clone(), us=us.clone(), uw=uw.clone(), Ms=Ms.to(self.device, torch.float64).clone(), ugt=None, nug=None)
+        self._static_labels(g, key[-2], targets)
+        if ugt is not None:          # with_gt: the unlabeled ground truth, capacity key[-1]
+            self._static_labels(g, key[-1], ugt, "ugt", "nug", "gcap")
         self.captures += 1
         return g
 
-    def _ssod_stage(self, g, imgs, targets, us, uw, Ms):
+    def _ssod_stage(self, g, imgs, targets, us, uw, Ms, ugt):
         g["imgs"].copy_(imgs, non_blocking=True)
         self._stage_labels(g, targets)
+        if ugt is not None:
+            self._stage_labels(g, ugt, "ugt", "nug")
         g["us"].copy_(us, non_blocking=True)
         g["uw"].copy_(uw, non_blocking=True)
         g["Ms"].copy_(Ms, non_blocking=True)
 
     def _ssod_body(self, g):
-        return self.train_instance(g["imgs"], g["targets"], g["us"], g["uw"], None, g["Ms"], None, _stop_after_backward=True,
-                                   _n_dev=g["nt"])
+        return self.train_instance(g["imgs"], g["targets"], g["us"], g["uw"], g["ugt"], g["Ms"], None, _stop_after_backward=True,
+                                   _n_dev=g["nt"], _m_dev=g["nug"])
 
     _SSOD_GRAPH = GraphHooks(_ssod_static, _ssod_stage, _ssod_body,
                              lambda self, scalars_dev: update_ema_pair(self.ema, self.semi_ema, self.model, scalars_dev=scalars_dev),
@@ -511,12 +554,17 @@ class SSODTrainerStep(TrainerStep):
         """train_instance captured once per image shape (device-resident pseudo labels, no host sync anywhere in the step)
         and replayed as two graphs (TrainerStep._graphed): A = teacher forward ... backward, B = SGD-Nesterov + both EMA
         updates.  The labels go into a static buffer of capacity C with their count on the device (_static_labels), so
-        any label count up to C replays the same graph; a batch with more re-captures once, with C doubled until it fits."""
+        any label count up to C replays the same graph; a batch with more re-captures once, with C doubled until it fits.
+        With with_gt, unlabeled_gt (None: no boxes) goes into a static buffer the same way, with its own capacity."""
         self._require_semi_ema()
         cap = self._label_capacity("_graph", targets, self.LABEL_CAPACITY)
+        ugt = None
+        if self.with_gt:
+            ugt = torch.zeros((0, 6)) if unlabeled_gt is None else unlabeled_gt.reshape(-1, 6)
+        gcap = 0 if ugt is None else self._label_capacity("_graph", ugt, self.LABEL_CAPACITY, "gcap")
         key = (tuple(imgs.shape), tuple(unlabeled_imgs.shape), tuple(unlabeled_M.shape),
-               imgs.dtype, unlabeled_imgs.dtype, unlabeled_imgs_ori.dtype, cap)   # uint8 loader batches vs fp32: different static buffers
-        loss = self._graphed("_graph", key, self._SSOD_GRAPH, (imgs, targets, unlabeled_imgs, unlabeled_imgs_ori, unlabeled_M), ni)
+               imgs.dtype, unlabeled_imgs.dtype, unlabeled_imgs_ori.dtype, cap, gcap)   # uint8 loader batches vs fp32: different static buffers
+        loss = self._graphed("_graph", key, self._SSOD_GRAPH, (imgs, targets, unlabeled_imgs, unlabeled_imgs_ori, unlabeled_M, ugt), ni)
         if hasattr(self.pseudo_label_creator, "stage_detections"):   # LabelMatch: the captured body neither stages nor counts
             self.pseudo_label_creator.stage_detections()
             self._count_labelmatch_images(imgs, unlabeled_imgs)
@@ -623,8 +671,8 @@ class SSODTrainerStep(TrainerStep):
 
     def _burn_in_step(self, imgs, targets, unlabeled_imgs_ori, ni):
         loss, items = self._burn_in_loss(imgs, targets, unlabeled_imgs_ori)
+        self._log(loss, items)
         self.update_optimizer(loss, ni)
-        self.last = dict(loss=loss.detach(), sup={k: v.detach() for k, v in items.items()})
         return loss.detach()
 
     def train_without_unlabeled(self, imgs, targets, ni):
@@ -673,7 +721,8 @@ class SSODTrainerStep(TrainerStep):
     def _burn_in_forward_backward(self, g):
         # returns the loss detached: nothing may keep this step's autograd graph alive, because the AccumulateGrad nodes of
         # the parameters it holds are tied to the stream they were created on (the warm-up's side stream, the capture's)
-        loss, _ = self._burn_in_loss(g["imgs"], g["targets"], g["uw"], g["nt"])
+        loss, items = self._burn_in_loss(g["imgs"], g["targets"], g["uw"], g["nt"])
+        self._log(loss, items)
         self._backward(loss)
         return loss.detach()
 
@@ -697,7 +746,8 @@ class SupTrainerStep(TrainerStep):
             self._bn_broadcast()      # DDP broadcast_buffers=True (captured steps: _graphed issues it before the replay)
         with torch.autocast("cuda", dtype=self.amp_dtype):
             pred = self.model(imgs)
-        loss, _ = self.compute_loss(pred, targets, n_dev)
+        loss, items = self.compute_loss(pred, targets, n_dev)
+        self._log(loss, items)
         return loss
 
     def train_step(self, imgs, targets, ni):

@@ -471,6 +471,33 @@ typedef struct EtbV8Levels {
 int etb_v8_decode(const float* cls, const float* reg, const EtbV8Levels* levels, int32_t B, int32_t nc, int32_t reg_max,
                   float grid_cell_offset, float* pred, float* boxes_grid, float* boxes_pix, float* scores, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Pseudo-label quality statistics of the SSOD step: utils/self_supervised_utils.py:481-587 check_pseudo_label_with_gt
+ * (with_gt = 1) and :589-606 check_pseudo_label (with_gt = 0), including their select_targets (:456-479) -- the host
+ * loops (one .cpu() per row, numpy matching) that trainer/ssod_trainer.py:661-670 runs every iteration.  Restated in
+ * csrc/plq.cu.  rows [cap,9] float64 pseudo labels, n from n_dev if non-NULL (capped at n_host), else n_host;
+ * thr_high / thr_low [nc] float64 (the ones etb_select_targets reads; both NULL: every row, with_gt only); gt [capG,6]
+ * fp32 (img, cls, x, y, w, h normalised), m from m_dev / m_host; iouv [T] float64 (T <= 16); batch_size > 0.
+ * iou64 = 1 (no thresholds, float64 rows): the IoU in float64 as torch promotes it.
+ * vals [5][T] float64: tp, fp_cls, fp_loc per threshold, then pse_num, gt_num (repeated over T), in the trainer's meaning
+ * (with_gt = 0: precision, 0, recall, reliable + uncertain, reliable); n == 0 gives all zeros (the invalid step).
+ * cnt [5 + 3T] int32: n, n_uncertain, n_reliable, m, overflow (1: an image with more than 1024 GT boxes, whose rest is
+ * ignored, a class index outside [0, nc) or a negative image index), then the tp, fp_cls and fp_loc counts [T] each.
+ * Two launches, no host sync; workspace: etb_pl_quality_workspace_bytes(), contents irrelevant on entry.
+ * ------------------------------------------------------------------------------------------- */
+size_t etb_pl_quality_workspace_bytes(void);
+int etb_pl_quality(const double* rows, const int32_t* n_dev, int32_t n_host, const double* thr_high, const double* thr_low,
+                   int32_t nc, const float* gt, const int32_t* m_dev, int32_t m_host, const double* iouv, int32_t T,
+                   int32_t batch_size, int32_t with_gt, int32_t iou64, double* vals, int32_t* cnt, void* workspace,
+                   size_t workspace_bytes, void* stream);
+
+/* MetricMeter / AverageMeter.update (utils/metrics.py:352-414) on the device: state [3][cap] float64 (sum, count, val);
+ * for each i < n (n <= ETB_METER_MAX_SRC, distinct slots): v = *src[i] (float64 if f64[i], else fp32 widened);
+ * sum[slot] += v; count[slot] += 1; val[slot] = v.  src / slot / f64 are host arrays.  One launch. */
+#define ETB_METER_MAX_SRC 16
+int etb_meter_update(double* state, int32_t cap, const void* const* src, const int32_t* slot, const int32_t* f64, int32_t n,
+                     void* stream);
+
 #ifdef __cplusplus
 }
 #endif
