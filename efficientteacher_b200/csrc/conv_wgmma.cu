@@ -14,9 +14,9 @@
 //   * both land in 128B-swizzled shared memory = the canonical K-major wgmma layout.
 //   * warpgroup roles: warpgroup 0 is the TMA producer (one elected lane of its first warp issues), warpgroups 1 and 2
 //     each own 64 of the 128 pixel rows and issue wgmma.m64nBNk16 x4 per stage; the fp32 accumulator lives in their
-//     registers, and the epilogue (folded BN scale/bias -> SiLU -> +residual -> bf16 NHWC store at a channel offset of a
-//     wider buffer, so torch.cat is free) runs straight from those registers; the raw-output epilogue (EPI 0) stages the
-//     tile in shared memory as bf16 and the producer warpgroup's second warp stores it by TMA (conv_store_warp).
+//     registers.  The bf16 epilogues (raw, or folded BN scale/bias -> SiLU -> +residual, stored at a channel offset of a
+//     wider buffer, so torch.cat is free) stage the tile in shared memory and the producer warpgroup's second warp stores
+//     it by TMA (conv_store_warp); only the Detect fp32 scatter and outputs with Cout % 8 != 0 store from registers.
 //   * every mbarrier wait is bounded (trap after ~2 s) so a descriptor bug cannot hang the GPU.
 #include "common.cuh"
 #include <cuda.h>
@@ -174,9 +174,12 @@ struct ConvKArgs {
   float* y_f32;
 };
 
-// EPI 0 stages the whole 128 x BN output tile as bf16 in the shared-memory image of the output tensor map's box
-// {64 ch, TW, TH, 1} under the 128 B swizzle: one 128-row x 128 B region per 64 channels (16 KB, 1024 B aligned), tile row
-// r = th*TW + tw, 16 B chunk q of row r at q ^ (r % 8).  32 KB at BN = 128, 16 KB at BN = 64.
+// The staged epilogues (EPI 0, 1, 3; see conv_epilogue) keep the whole 128 x BN output tile as bf16 in the shared-memory
+// image of the output tensor map's box {64 ch, TW, TH, 1} under the 128 B swizzle: one 128-row x 128 B region per 64
+// channels (16 KB, 1024 B aligned), tile row r = th*TW + tw, 16 B chunk q of row r at q ^ (r % 8).  32 KB at BN = 128,
+// 16 KB at BN = 64.
+__host__ __device__ constexpr bool conv_staged(int epi) { return epi == 0 || epi == 1 || epi == 3; }
+
 template <int BN, int EPI>
 struct ConvSmem {
   static constexpr int A_BYTES = CONV_BLOCK_M * 128;
@@ -184,7 +187,7 @@ struct ConvSmem {
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int STAGES = CONV_SMEM_STAGES_BYTES / STAGE_BYTES;   // 6 (BN = 128) or 8 (BN = 64)
   static constexpr int OUT_REGION = CONV_BLOCK_M * 128;                 // one 64-channel region of the staged tile
-  static constexpr int OUT_BYTES = EPI == 0 ? (BN / 64) * OUT_REGION : 0;
+  static constexpr int OUT_BYTES = conv_staged(EPI) ? (BN / 64) * OUT_REGION : 0;
   static constexpr int OUT_OFF = STAGES * STAGE_BYTES;
   static constexpr int BAR_OFF = OUT_OFF + OUT_BYTES;
   static constexpr int TOTAL = BAR_OFF + 256 + 1024;        // + barriers + slack for the 1024 B alignment
@@ -198,16 +201,23 @@ __device__ __forceinline__ float conv_act(float x, int act) {
   return x;
 }
 
-// Epilogue of one consumer warpgroup's 64 x BN accumulator, straight from the wgmma fragment (see wgmma_m64n*k16): this
-// thread owns pixel rows r0 and r0+8 and, per 8-column block j, the channel pair 8j + 2*(lane%4) + {0,1}.  EPI selects the
-// fused tail at compile time so every register array is statically indexed (EPI 0 is conv_epilogue_stage below):
-//   EPI 0: raw bf16 store (+= existing when a.accumulate)       -- dgrad, training forward (conv_epilogue_stage)
-//   EPI 1: v*scale+bias (folded BN) -> SiLU/ReLU -> (+residual) -- teacher forward
-//   EPI 2: +bias, fp32 scatter into the Detect layout           -- head
-//   EPI 3: EPI 1 with Hardswish                                 -- teacher forward of Hardswish layers
-// (Hardswish as a third run-time case of EPI 1 would raise the SiLU instances from 122 / 89 to 132 / 98 registers.)
-template <int BN, int EPI>
+// Epilogue instances.  EPI selects the tail at compile time so every register array is statically indexed:
+//   EPI 0: raw bf16 (+= existing when a.accumulate)               -- dgrad, training forward       staged
+//   EPI 1: v*scale+bias (folded BN) -> SiLU/ReLU -> (+residual)   -- teacher forward               staged
+//   EPI 2: +bias, fp32 scatter into the Detect layout             -- head                          registers
+//   EPI 3: EPI 1 with Hardswish                                   -- teacher forward, Hardswish    staged
+//   EPI 4: bf16 with Cout % 8 != 0: EPI 1/3 without the shortcut  -- netD's 2-channel output,      registers
+//          (a raw output is scale 1, bias 0, no activation)          the raw head of 255 channels
+// The staged ones go through shared memory and a TMA store (conv_epilogue_stage, conv_store_warp), which writes whole
+// 16 B channel groups; the others store from registers (conv_epilogue).  Hardswish has its own staged instance because a
+// third run-time case in EPI 1 costs the SiLU instances registers; EPI 4 picks its Hardswish body (HS) once per tile, as a
+// per-element choice would put the division's slow path into the SiLU loop.
+//
+// Register path: one consumer warpgroup's 64 x BN accumulator, straight from the wgmma fragment (see wgmma_m64n*k16): this
+// thread owns pixel rows r0 and r0+8 and, per 8-column block j, the channel pair 8j + 2*(lane%4) + {0,1}.
+template <int BN, int EPI, bool HS>
 __device__ __forceinline__ void conv_epilogue(const ConvKArgs& a, const float* d, int n0, const bool* row_ok, const size_t* pix, int lane) {
+  static_assert(EPI == 2 || EPI == 4, "EPI 0, 1 and 3 are staged");
   const size_t hw = (size_t)a.det_hw;
   const int na = EPI == 2 ? a.Cout / a.det_no : 1;
 #pragma unroll
@@ -216,8 +226,8 @@ __device__ __forceinline__ void conv_epilogue(const ConvKArgs& a, const float* d
     if (gc >= a.Cout) continue;
     const bool pair = gc + 1 < a.Cout;
     float sc0 = 1.f, sc1 = 1.f, bi0 = 0.f, bi1 = 0.f;
-    if ((EPI == 1 || EPI == 3) && a.scale) { sc0 = __ldg(a.scale + gc); sc1 = pair ? __ldg(a.scale + gc + 1) : 1.f; }
-    if (EPI != 0 && a.bias) { bi0 = __ldg(a.bias + gc); bi1 = pair ? __ldg(a.bias + gc + 1) : 0.f; }
+    if (EPI == 4 && a.scale) { sc0 = __ldg(a.scale + gc); sc1 = pair ? __ldg(a.scale + gc + 1) : 1.f; }
+    if (a.bias) { bi0 = __ldg(a.bias + gc); bi1 = pair ? __ldg(a.bias + gc + 1) : 0.f; }
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
       if (!row_ok[i]) continue;
@@ -234,15 +244,10 @@ __device__ __forceinline__ void conv_epilogue(const ConvKArgs& a, const float* d
         continue;
       }
       __nv_bfloat16* yp = a.y + pix[i] * a.y_cstride + a.y_coffset + gc;
-      if (EPI == 1 || EPI == 3) {
-        v0 = EPI == 3 ? hswish_f(fmaf(v0, sc0, bi0)) : conv_act(fmaf(v0, sc0, bi0), a.act);
-        v1 = EPI == 3 ? hswish_f(fmaf(v1, sc1, bi1)) : conv_act(fmaf(v1, sc1, bi1), a.act);
-        if (a.residual) {     // Cout % 8 == 0 whenever a shortcut is fused: the pair is whole
-          const float2 rf = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(a.residual + pix[i] * a.res_cstride + a.res_coffset + gc));
-          v0 += rf.x;
-          v1 += rf.y;
-        }
-      }
+      v0 = fmaf(v0, sc0, bi0);
+      v1 = fmaf(v1, sc1, bi1);
+      v0 = HS ? hswish_f(v0) : conv_act(v0, a.act);
+      v1 = HS ? hswish_f(v1) : conv_act(v1, a.act);
       if (pair) *reinterpret_cast<__nv_bfloat162*>(yp) = __floats2bfloat162_rn(v0, v1);
       else *yp = __float2bfloat16(v0);
     }
@@ -276,24 +281,45 @@ __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.comm
 __device__ __forceinline__ void bulk_wait_read_all() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
 __device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
-// EPI 0, consumer side: this thread's fragment (rows r and r+8, channel pair 8j + 2*(lane%4) per 8-column block j; see
-// wgmma_m64n*k16) goes into the staged tile `stg` (ConvSmem layout) as bf16 pairs.  With a.accumulate the staged tile
-// already holds the tile's existing output (TMA-loaded by the store warp) and each pair is read, added in fp32 and rounded
-// once, which is the value of old + acc rounded once.  Regions that lie wholly past Cout are neither loaded nor stored.
+// The staged tile is prefetched with a second operand of the epilogue: EPI 0's existing output (a.accumulate, the
+// gradient fan-in) or EPI 1/3's shortcut (a.residual), both read in place and added in fp32 before the one rounding.
+template <int EPI>
+__device__ __forceinline__ bool conv_prefetch(const ConvKArgs& a) {
+  return EPI == 0 ? a.accumulate != 0 : a.residual != nullptr;
+}
+
+// Staged epilogue, consumer side: this thread's fragment (rows r and r+8, channel pair 8j + 2*(lane%4) per 8-column block
+// j; see wgmma_m64n*k16) goes into the staged tile `stg` (ConvSmem layout) as bf16 pairs: the raw value (EPI 0) or
+// act(v*scale + bias) (EPI 1/3).  With a prefetched operand (conv_prefetch) the staged tile already holds it (TMA-loaded
+// by the store warp) and each pair is read, added in fp32 and rounded once, which is the value of old + acc (EPI 0) or
+// act(...) + shortcut (EPI 1/3) rounded once.  Regions that lie wholly past Cout are neither loaded nor stored; EPI 1/3
+// also skip the 8-column blocks past Cout (their scale and bias do not exist; Cout % 8 == 0 keeps the test uniform).
 // A warp's 4 B accesses cover 8 consecutive rows x 4 lanes: the swizzle puts the 8 rows in 8 distinct 16 B chunks, so
 // they are free of bank conflicts.
-template <int BN>
+template <int BN, int EPI>
 __device__ __forceinline__ void conv_epilogue_stage(const ConvKArgs& a, const float* d, int n0, int row, int lane, uint32_t stg) {
+  static_assert(conv_staged(EPI), "EPI 2 and 4 store from registers");
   const uint32_t base = stg + row * 128 + 4 * (lane & 3);
   const int sw = row & 7;                      // also the swizzle of row + 8
+  const bool pre = conv_prefetch<EPI>(a);
 #pragma unroll
   for (int j = 0; j < BN / 8; ++j) {
-    if ((j & 7) == 0 && n0 + 8 * j >= a.Cout) break;     // uniform: the region lies beyond Cout
+    if (EPI == 0 ? ((j & 7) == 0 && n0 + 8 * j >= a.Cout) : n0 + 8 * j >= a.Cout) break;   // uniform, past Cout
+    float sc0 = 1.f, sc1 = 1.f, bi0 = 0.f, bi1 = 0.f;
+    if (EPI != 0) {
+      const int gc = n0 + 8 * j + 2 * (lane & 3);
+      if (a.scale) { sc0 = __ldg(a.scale + gc); sc1 = __ldg(a.scale + gc + 1); }
+      if (a.bias) { bi0 = __ldg(a.bias + gc); bi1 = __ldg(a.bias + gc + 1); }
+    }
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
-      const uint32_t addr = base + (j >> 3) * ConvSmem<BN, 0>::OUT_REGION + i * 8 * 128 + (((j & 7) ^ sw) << 4);
+      const uint32_t addr = base + (j >> 3) * ConvSmem<BN, EPI>::OUT_REGION + i * 8 * 128 + (((j & 7) ^ sw) << 4);
       float v0 = d[j * 4 + i * 2], v1 = d[j * 4 + i * 2 + 1];
-      if (a.accumulate) {
+      if (EPI != 0) {
+        v0 = EPI == 3 ? hswish_f(fmaf(v0, sc0, bi0)) : conv_act(fmaf(v0, sc0, bi0), a.act);
+        v1 = EPI == 3 ? hswish_f(fmaf(v1, sc1, bi1)) : conv_act(fmaf(v1, sc1, bi1), a.act);
+      }
+      if (pre) {
         const uint32_t old = ld_shared_u32(addr);
         const float2 f = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&old));
         v0 += f.x;
@@ -305,18 +331,23 @@ __device__ __forceinline__ void conv_epilogue_stage(const ConvKArgs& a, const fl
   }
 }
 
-// EPI 0, store side: warp 1 walks the CTA's tiles in the consumers' order, one lane issuing (bulk groups belong to the
-// issuing thread).  Per tile:
-//   a.accumulate: TMA-load the tile's existing output into the staged tile (free: first tile, or the previous tile's
-//     stores have finished reading it) -> acc_full; this runs while the consumers are in the tile's K loop;
+// Staged epilogue, store side: warp 1 walks the CTA's tiles in the consumers' order, one lane issuing (bulk groups belong
+// to the issuing thread).  Per tile:
+//   with a prefetched operand: TMA-load the tile's existing output (mapY, EPI 0) or shortcut (mapR, EPI 1/3) into the
+//     staged tile (free: first tile, or the previous tile's stores have finished reading it) -> acc_full; this runs
+//     while the consumers are in the tile's K loop;
 //   wait stg_full (all 256 consumer threads have written the tile and fenced) -> one bulk tensor store per 64-channel
 //   region inside Cout -> wait until the stores have read shared memory -> stg_empty.
 // The consumers wait for stg_empty only before they next write the tile, a whole K loop later.  TMA clips every box
-// at Cout, at the edges of the output lattice and at the last pixel, so nothing outside the output is written.
-template <int BN>
-__device__ __forceinline__ void conv_store_warp(const CUtensorMap* mapY, const ConvKArgs& a, uint8_t* stg, uint64_t* stg_full,
-                                                uint64_t* stg_empty, uint64_t* acc_full, int n_tiles, int total_tiles) {
+// at Cout, at the edges of the output lattice and at the last pixel, so nothing outside the output is written (and the
+// loads fill what lies outside with zeros).
+template <int BN, int EPI>
+__device__ __forceinline__ void conv_store_warp(const CUtensorMap* mapY, const CUtensorMap* mapR, const ConvKArgs& a, uint8_t* stg,
+                                                uint64_t* stg_full, uint64_t* stg_empty, uint64_t* acc_full, int n_tiles,
+                                                int total_tiles) {
   const bool leader = (threadIdx.x & 31) == 0;
+  const bool pre = conv_prefetch<EPI>(a);
+  const CUtensorMap* mapP = EPI == 0 ? mapY : mapR;
   uint32_t ph = 0;
   for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ph ^= 1u) {
     const int n0 = (tile % n_tiles) * BN;
@@ -325,9 +356,9 @@ __device__ __forceinline__ void conv_store_warp(const CUtensorMap* mapY, const C
     const int th_i = t % a.tiles_h; t /= a.tiles_h;
     const int c1 = tw_i * a.TW, c2 = th_i * a.TH, img = t;
     const int nreg = min(BN / 64, (a.Cout - n0 + 63) / 64);
-    if (a.accumulate && leader) {
+    if (pre && leader) {
       mbar_expect_tx(acc_full, (uint32_t)(nreg * a.TW * a.TH * 128));
-      for (int r = 0; r < nreg; ++r) tma_load_4d(mapY, acc_full, stg + r * ConvSmem<BN, 0>::OUT_REGION, n0 + 64 * r, c1, c2, img);
+      for (int r = 0; r < nreg; ++r) tma_load_4d(mapP, acc_full, stg + r * ConvSmem<BN, EPI>::OUT_REGION, n0 + 64 * r, c1, c2, img);
     }
     mbar_wait(stg_full, ph);
     if (leader) {
@@ -343,22 +374,23 @@ __device__ __forceinline__ void conv_store_warp(const CUtensorMap* mapY, const C
 
 // Persistent: gridDim.x CTAs walk the tile list (tile = blockIdx.x + i*gridDim.x; N tile fastest so the CTAs running
 // concurrently share A tiles in L2).  The smem ring runs across tile boundaries, so the producer streams the operands of
-// tile i+1 while the consumers run the epilogue of tile i.  EPI 0 hands each tile to the store warp (conv_store_warp) through
-// the staged tile in shared memory and goes straight on to the next tile's K loop; mapY is its output map (unused by
-// EPI 1-3, which store from registers).
+// tile i+1 while the consumers run the epilogue of tile i.  The staged instances (EPI 0, 1, 3) hand each tile to the store
+// warp (conv_store_warp) through the staged tile in shared memory and go straight on to the next tile's K loop; mapY is
+// their output map and mapR the shortcut map of EPI 1/3 (both unused by EPI 2 and 4, which store from registers).
 template <int BN, int EPI>
 __global__ void __launch_bounds__(CONV_THREADS, 1)
 conv_fwd_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB,
-                const __grid_constant__ CUtensorMap mapY, const ConvKArgs a) {
+                const __grid_constant__ CUtensorMap mapY, const __grid_constant__ CUtensorMap mapR, const ConvKArgs a) {
   using L = ConvSmem<BN, EPI>;
   constexpr int STAGES = L::STAGES;
+  constexpr bool STAGED = conv_staged(EPI);
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   uint64_t* full = (uint64_t*)(smem + L::BAR_OFF);
   uint64_t* empty = full + STAGES;
-  uint64_t* stg_full = empty + STAGES;     // EPI 0: consumers -> store warp, the staged tile is written
-  uint64_t* stg_empty = stg_full + 1;      //        store warp -> consumers, the stores have read it
-  uint64_t* acc_full = stg_full + 2;       //        store warp -> consumers, the existing output is loaded (a.accumulate)
+  uint64_t* stg_full = empty + STAGES;     // staged: consumers -> store warp, the staged tile is written
+  uint64_t* stg_empty = stg_full + 1;      //         store warp -> consumers, the stores have read it
+  uint64_t* acc_full = stg_full + 2;       //         store warp -> consumers, the prefetched operand is loaded (conv_prefetch)
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int wg = warp >> 2;
@@ -371,8 +403,9 @@ conv_fwd_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
     tma_prefetch_desc(&mapA);
     tma_prefetch_desc(&mapB);
     for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }   // 8 consumer warps release a stage
-    if (EPI == 0) {
+    if (STAGED) {
       tma_prefetch_desc(&mapY);
+      if (EPI != 0 && a.residual) tma_prefetch_desc(&mapR);
       mbar_init(stg_full, 256);
       mbar_init(stg_empty, 1);
       mbar_init(acc_full, 1);
@@ -382,8 +415,8 @@ conv_fwd_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
   __syncthreads();
 
   if (wg == 0) {
-    if (EPI == 0 && warp == 1) {
-      conv_store_warp<BN>(&mapY, a, smem + L::OUT_OFF, stg_full, stg_empty, acc_full, n_tiles, total_tiles);
+    if (STAGED && warp == 1) {
+      conv_store_warp<BN, EPI>(&mapY, &mapR, a, smem + L::OUT_OFF, stg_full, stg_empty, acc_full, n_tiles, total_tiles);
       return;
     }
     if (warp != 0) return;
@@ -424,7 +457,7 @@ conv_fwd_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
   float d[BN / 2];
   int s = 0;
   uint32_t ph = 0;
-  uint32_t tph = 0;                // EPI 0: parity of the staged-tile barriers, one phase per tile
+  uint32_t tph = 0;                // staged: parity of the staged-tile barriers, one phase per tile
   for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
     int prev = -1;
     for (int ki = 0; ki < kiters; ++ki) {
@@ -445,10 +478,10 @@ conv_fwd_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
     acc_fence<BN / 2>(d);
     if (lane == 0) mbar_arrive(&empty[prev]);
     const int n0 = (tile % n_tiles) * BN;
-    if constexpr (EPI == 0) {
+    if constexpr (STAGED) {
       mbar_wait(stg_empty, tph ^ 1u);          // the previous tile's stores have read the staged tile
-      if (a.accumulate) mbar_wait(acc_full, tph);
-      conv_epilogue_stage<BN>(a, d, n0, rbase, lane, smem_u32(smem + L::OUT_OFF));
+      if (conv_prefetch<EPI>(a)) mbar_wait(acc_full, tph);
+      conv_epilogue_stage<BN, EPI>(a, d, n0, rbase, lane, smem_u32(smem + L::OUT_OFF));
       fence_proxy_async_smem();
       mbar_arrive(stg_full);
       tph ^= 1u;
@@ -461,7 +494,8 @@ conv_fwd_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
       size_t pix[2];
 #pragma unroll
       for (int i = 0; i < 2; ++i) row_ok[i] = conv_out_pixel(a, img, th_i, tw_i, rbase + 8 * i, &pix[i]);
-      conv_epilogue<BN, EPI>(a, d, n0, row_ok, pix, lane);
+      if (EPI == 4 && a.act == 4) conv_epilogue<BN, EPI, true>(a, d, n0, row_ok, pix, lane);
+      else conv_epilogue<BN, EPI, false>(a, d, n0, row_ok, pix, lane);
     }
   }
 }
@@ -497,35 +531,37 @@ static void pick_tile(int Wo, int Ho, int* TW, int* TH) {
 }
 
 template <int BN, int EPI>
-static int launch_conv_e(const CUtensorMap& mA, const CUtensorMap& mB, const CUtensorMap& mY, const ConvKArgs& ka, dim3 grid,
-                         cudaStream_t st) {
+static int launch_conv_e(const CUtensorMap& mA, const CUtensorMap& mB, const CUtensorMap& mY, const CUtensorMap& mR, const ConvKArgs& ka,
+                         dim3 grid, cudaStream_t st) {
   using L = ConvSmem<BN, EPI>;
   static bool attr_set = false;
   if (!attr_set) {
     ETB_CHECK_CUDA(cudaFuncSetAttribute(conv_fwd_kernel<BN, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::TOTAL));
     attr_set = true;
   }
-  etb_launch(conv_fwd_kernel<BN, EPI>, dim3(grid), dim3(CONV_THREADS), L::TOTAL, st, mA, mB, mY, ka);
+  etb_launch(conv_fwd_kernel<BN, EPI>, dim3(grid), dim3(CONV_THREADS), L::TOTAL, st, mA, mB, mY, mR, ka);
   ETB_CHECK_LAUNCH();
   return ETB_OK;
 }
-// The epilogue instance a launch runs (see conv_epilogue).  EPI 0's TMA store writes whole 16 B channel groups (the box
-// is not clipped inside one), so a raw output whose Cout is not a multiple of 8 goes through EPI 1 with scale 1, bias 0
-// and no activation, which stores the same values from registers channel by channel (no trunk width needs it).
+// The epilogue instance a launch runs (see conv_epilogue).  The TMA store of the staged instances writes whole 16 B
+// channel groups (the box is not clipped inside one), so a bf16 output whose Cout is not a multiple of 8 (netD's 2
+// channels, a raw 255-channel head; no trunk width) runs EPI 4, which stores the same values from registers.
 static int conv_epi(const ConvKArgs& ka) {
   if (ka.out_mode == 1) return 2;
+  if (ka.Cout % 8 != 0) return 4;
   if (ka.act == 4) return 3;
-  if (ka.scale || ka.bias || ka.act || ka.residual || ka.Cout % 8 != 0) return 1;
+  if (ka.scale || ka.bias || ka.act || ka.residual) return 1;
   return 0;
 }
 template <int BN>
-static int launch_conv(const CUtensorMap& mA, const CUtensorMap& mB, const CUtensorMap& mY, const ConvKArgs& ka, dim3 grid,
-                       cudaStream_t st) {
+static int launch_conv(const CUtensorMap& mA, const CUtensorMap& mB, const CUtensorMap& mY, const CUtensorMap& mR, const ConvKArgs& ka,
+                       dim3 grid, cudaStream_t st) {
   switch (conv_epi(ka)) {
-    case 2: return launch_conv_e<BN, 2>(mA, mB, mY, ka, grid, st);
-    case 3: return launch_conv_e<BN, 3>(mA, mB, mY, ka, grid, st);
-    case 1: return launch_conv_e<BN, 1>(mA, mB, mY, ka, grid, st);
-    default: return launch_conv_e<BN, 0>(mA, mB, mY, ka, grid, st);
+    case 2: return launch_conv_e<BN, 2>(mA, mB, mY, mR, ka, grid, st);
+    case 4: return launch_conv_e<BN, 4>(mA, mB, mY, mR, ka, grid, st);
+    case 3: return launch_conv_e<BN, 3>(mA, mB, mY, mR, ka, grid, st);
+    case 1: return launch_conv_e<BN, 1>(mA, mB, mY, mR, ka, grid, st);
+    default: return launch_conv_e<BN, 0>(mA, mB, mY, mR, ka, grid, st);
   }
 }
 
@@ -602,31 +638,42 @@ static int launch_gemm(const GemmGeom& g, ConvKArgs ka, cudaStream_t st) {
   ka.kblocks = aCp / CONV_BLOCK_K;
   ka.Cout = g.b_rows;
   ka.nimg = nimg;
-  // EPI 0 output map: the Ho x Wo output lattice (pixel (oh,ow) at (oh*out_os+out_ph, ow*out_os+out_pw) of the out_H x
-  // out_W plane) inside the channel slice [y_coffset, +Cout) of y, box = one 64-channel region of the staged tile.  The
-  // flat tiling is the lattice 1 x npix.  All strides are multiples of 16 B (y_cstride % 8 == 0).
-  CUtensorMap mY;
-  memset(&mY, 0, sizeof(mY));
-  ETB_CHECK_ARG(!ka.accumulate || conv_epi(ka) == 0);   // only EPI 0 accumulates
-  if (conv_epi(ka) == 0) {
-    const cuuint64_t cs = (cuuint64_t)ka.y_cstride * 2;
-    cuuint64_t ydim[4] = {(cuuint64_t)ka.Cout, (cuuint64_t)ka.Wo, (cuuint64_t)ka.Ho, (cuuint64_t)nimg};
-    cuuint64_t ystr[3] = {cs * ka.out_os, cs * ka.out_os * ka.out_W, cs * ka.out_W * ka.out_H};
-    cuuint32_t ybox[4] = {64, (cuuint32_t)ka.TW, (cuuint32_t)ka.TH, 1};
-    cuuint32_t yestr[4] = {1, 1, 1, 1};
-    __nv_bfloat16* ybase = ka.y + ((size_t)ka.out_ph * ka.out_W + ka.out_pw) * ka.y_cstride + ka.y_coffset;
-    ETB_CHECK_ARG((((uintptr_t)ybase) & 15) == 0);
-    r = enc(&mY, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, ybase, ydim, ystr, ybox, yestr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-            CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) {
-      etb_set_error("cuTensorMapEncodeTiled(Y) failed: %d", (int)r);
+  // Maps of the staged epilogues: the Ho x Wo output lattice (pixel (oh,ow) at (oh*out_os+out_ph, ow*out_os+out_pw) of
+  // the out_H x out_W plane) inside a channel slice [coffset, +Cout) of a bf16 NHWC tensor, box = one 64-channel region
+  // of the staged tile.  The flat tiling is the lattice 1 x npix.  mY is the output (y_cstride, y_coffset); mR, for EPI
+  // 1/3 with a shortcut, the shortcut (res_cstride, res_coffset) on the same lattice.  All strides are multiples of 16 B
+  // (cstride % 8 == 0).
+  auto lattice_map = [&](CUtensorMap* m, const __nv_bfloat16* t, int cstride, int coffset, const char* what) -> int {
+    const cuuint64_t cs = (cuuint64_t)cstride * 2;
+    cuuint64_t dim[4] = {(cuuint64_t)ka.Cout, (cuuint64_t)ka.Wo, (cuuint64_t)ka.Ho, (cuuint64_t)nimg};
+    cuuint64_t str[3] = {cs * ka.out_os, cs * ka.out_os * ka.out_W, cs * ka.out_W * ka.out_H};
+    cuuint32_t mbox[4] = {64, (cuuint32_t)ka.TW, (cuuint32_t)ka.TH, 1};
+    cuuint32_t mestr[4] = {1, 1, 1, 1};
+    const __nv_bfloat16* base = t + ((size_t)ka.out_ph * ka.out_W + ka.out_pw) * cstride + coffset;
+    ETB_CHECK_ARG((((uintptr_t)base) & 15) == 0);
+    const CUresult rc = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<__nv_bfloat16*>(base), dim, str, mbox, mestr,
+                            CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (rc != CUDA_SUCCESS) {
+      etb_set_error("cuTensorMapEncodeTiled(%s) failed: %d", what, (int)rc);
       return ETB_ERR_CUDA;
     }
+    return ETB_OK;
+  };
+  CUtensorMap mY, mR;
+  memset(&mY, 0, sizeof(mY));
+  memset(&mR, 0, sizeof(mR));
+  const int epi = conv_epi(ka);
+  ETB_CHECK_ARG(!ka.accumulate || epi == 0);   // only EPI 0 accumulates
+  if (conv_staged(epi)) {
+    int rc = lattice_map(&mY, ka.y, ka.y_cstride, ka.y_coffset, "Y");
+    if (rc == ETB_OK && ka.residual) rc = lattice_map(&mR, ka.residual, ka.res_cstride, ka.res_coffset, "R");
+    if (rc != ETB_OK) return rc;
   }
   const long total_tiles = (long)ka.tiles_w * ka.tiles_h * nimg * ((g.b_rows + BN - 1) / BN);
   const long resident = (long)etb_num_sms();   // persistent: one CTA per SM (the operand ring takes 192 KB of shared memory)
   dim3 grid((unsigned)(total_tiles < resident ? total_tiles : resident), 1);
-  return BN == 128 ? launch_conv<128>(mA, mB, mY, ka, grid, st) : launch_conv<64>(mA, mB, mY, ka, grid, st);
+  return BN == 128 ? launch_conv<128>(mA, mB, mY, mR, ka, grid, st) : launch_conv<64>(mA, mB, mY, mR, ka, grid, st);
 }
 
 extern "C" int etb_conv_fwd(const void* x_bf16, const void* w_bf16, const float* scale, const float* bias,
@@ -640,7 +687,9 @@ extern "C" int etb_conv_fwd(const void* x_bf16, const void* w_bf16, const float*
   ETB_CHECK_ARG(Ho > 0 && Wo > 0);
   const bool det = (y_f32 != nullptr);
   if (!det) ETB_CHECK_ARG(cp->y_cstride % 8 == 0 && cp->y_coffset % 8 == 0 && cp->y_cstride >= cp->y_coffset + cp->Cout && (((uintptr_t)y_bf16) & 15) == 0);
-  if (residual_bf16) ETB_CHECK_ARG(!det && cp->res_cstride % 8 == 0 && cp->res_coffset % 8 == 0 && cp->Cout % 8 == 0);
+  // the shortcut is TMA-loaded with the output's box (launch_gemm): whole 16 B channel groups of a 16 B-aligned slice
+  if (residual_bf16) ETB_CHECK_ARG(!det && cp->res_cstride % 8 == 0 && cp->res_coffset % 8 == 0 && cp->Cout % 8 == 0 &&
+                                   cp->res_cstride >= cp->res_coffset + cp->Cout && (((uintptr_t)residual_bf16) & 15) == 0);
   if (det) ETB_CHECK_ARG(cp->det_no > 0 && cp->Cout % cp->det_no == 0);
   ConvKArgs ka;
   memset(&ka, 0, sizeof(ka));

@@ -1,6 +1,7 @@
 """Per-layer-shape timing of the wgmma conv kernels on the YOLOv5l@640 shapes, CUDA events, L2 flushed between iterations.
-Modes: fwd (folded BN + SiLU), raw (raw output: the student's training forward), dgrad, dgrad_acc (dgrad added into the
-existing input gradient: gradient fan-in), wgrad.
+Modes: fwd (folded BN + SiLU), fwd_res (folded BN + SiLU + shortcut: the Bottleneck's second conv, on the 3x3 s1 C->C
+shapes only), raw (raw output: the student's training forward), dgrad, dgrad_acc (dgrad added into the existing input
+gradient: gradient fan-in), wgrad.
   python tools/conv_bench.py [--batch 16] [--modes fwd,dgrad,wgrad] [--out bench_out/conv_bench.json]"""
 import argparse
 import json
@@ -103,6 +104,14 @@ def main():
             ms = timeit(lambda: co.conv_fwd(x, wp, Cin, Cout, k, s, p, sc, bi, "silu", out=y))
             row["fwd_us"], row["fwd_tflops"] = ms * 1e3, flops / ms / 1e9
             tot["fwd"][0] += ms * cnt; tot["fwd"][1] += flops * cnt
+        if "fwd_res" in tot and name.startswith("3x3"):   # Bottleneck cv2: the shortcut is added in the epilogue
+            wp = co.pack_weight(w)
+            sc = torch.ones(Cout, device=dev); bi = torch.zeros(Cout, device=dev)
+            y = torch.empty(N, Ho, Ho, cpad, dtype=torch.bfloat16, device=dev)
+            r = torch.randn(N, Ho, Ho, cpad, device=dev).to(torch.bfloat16)
+            ms = timeit(lambda: co.conv_fwd(x, wp, Cin, Cout, k, s, p, sc, bi, "silu", out=y, residual=r))
+            row["fwd_res_us"], row["fwd_res_tflops"] = ms * 1e3, flops / ms / 1e9
+            tot["fwd_res"][0] += ms * cnt; tot["fwd_res"][1] += flops * cnt
         if "raw" in tot:        # the student's training forward: raw bf16 conv output (BN statistics come next)
             wp = co.pack_weight(w)
             y = torch.empty(N, Ho, Ho, cpad, dtype=torch.bfloat16, device=dev)
