@@ -54,7 +54,9 @@ class EtbLossParams(C.Structure):
                 ("nx", C.c_int32 * ETB_MAX_LEVELS), ("ny", C.c_int32 * ETB_MAX_LEVELS),
                 ("balance", C.c_float * ETB_MAX_LEVELS), ("box_w", C.c_float), ("obj_w", C.c_float),
                 ("cls_w", C.c_float), ("cp", C.c_float), ("cn", C.c_float), ("nsets", C.c_int32),
-                ("ignore_obj", C.c_int32), ("with_bbox", C.c_int32), ("with_cls", C.c_int32)]
+                ("ignore_obj", C.c_int32), ("with_bbox", C.c_int32), ("with_cls", C.c_int32),
+                ("cls_pw", C.c_float), ("obj_pw", C.c_float), ("fl_gamma", C.c_float), ("ssi", C.c_int32),
+                ("balance_state", vp)]
 
 
 class EtbPackDesc(C.Structure):

@@ -39,10 +39,12 @@ class AssignBuffers:
 class YOLOAnchorAssigner:
     def __init__(self, na, nl, anchors, anchor_t, stride, nc=80, num_keypoints=0, single_targets=False, ota=False,
                  top_k=10):
-        if num_keypoints or ota or single_targets:
+        if num_keypoints or ota:
             raise NotImplementedError("efficientteacher_b200: only build_targets / build_uc_targets_aug are on the "
-                                      "hot path (SURVEY.md section 8 a9); OTA / keypoint / single-target "
-                                      "assigners are out of scope")
+                                      "hot path (SURVEY.md section 8 a9); OTA / keypoint assigners are out of scope")
+        # single_targets is stored and never read, as in the reference (yolo_anchor_assigner.py:34-51): its
+        # build_single_targets is unreachable, so single_targets=True assigns exactly as the default does
+        self.single_targets = single_targets
         self.na, self.nl, self.anchors, self.anchor_t = na, nl, anchors, anchor_t
         self.nc, self.np, self.stride, self.ota, self.top_k = nc, num_keypoints, stride, ota, top_k
         assert na == 3 and 1 <= nl <= ETB_MAX_LEVELS

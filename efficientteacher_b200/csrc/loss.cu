@@ -10,6 +10,10 @@
 // reference's CPU index_put_ does (SURVEY.md Appendix C #8); uncertain soft labels override certain ones
 // because the reference writes them later (ssod_loss.py:242-248).
 //
+// Loss options (cfg.Loss.cls_pw / obj_pw / fl_gamma, loss.py:106-116) change only the per-element criterion
+// (etb_det_bce in loss_math.h); autobalance (loss.py:191-197) keeps its double balance state on the device and
+// advances it in loss_finalize_kernel, so no call reads anything back to the host.
+//
 // HBM traffic (algorithmic): forward reads one objectness logit per cell (32 B sector each, B*P*32 B) plus
 // 85 floats per matched row; backward writes the dense gradient once (B*P*no*4 B).
 #include "common.cuh"
@@ -30,6 +34,7 @@ struct LossWs {
   int32_t* winner_c;  // [cells_total]
   int32_t* winner_u;  // [cells_total]
   float* iou0;        // [nl][cap0]
+  float* bal_used;    // [nl] autobalance: the float32 balance this call's forward used, for its backward
   int64_t cell_off[ETB_MAX_LEVELS + 1];
   int32_t cap0;
 };
@@ -54,11 +59,13 @@ static size_t loss_layout(const EtbLossParams* lp, int32_t cap, char* base, Loss
   size_t o_wc = o;  o = lalign(o + sizeof(int32_t) * cells);
   size_t o_wu = o;  o = lalign(o + sizeof(int32_t) * cells);
   size_t o_iou = o; o = lalign(o + sizeof(float) * (size_t)cap * lp->nl);
+  size_t o_bal = o; o = lalign(o + sizeof(float) * lp->nl);
   if (ws) {
     ws->acc = (double*)(base + o_acc);
     ws->winner_c = (int32_t*)(base + o_wc);
     ws->winner_u = (int32_t*)(base + o_wu);
     ws->iou0 = (float*)(base + o_iou);
+    ws->bal_used = (float*)(base + o_bal);
     for (int l = 0; l <= lp->nl; ++l) ws->cell_off[l] = off[l];
     ws->cap0 = cap;
   }
@@ -135,7 +142,7 @@ __global__ void __launch_bounds__(256) loss_rows_kernel(LossPtrs P, EtbLossParam
           float csum = 0.f;
           if (do_cls) {
             const int tc = S.tcls[s][l][r];
-            for (int c = lane; c < nc; c += 32) csum += etb_bce_logits(ps[5 + c], c == tc ? lp.cp : lp.cn);
+            for (int c = lane; c < nc; c += 32) csum += etb_det_bce(ps[5 + c], c == tc ? lp.cp : lp.cn, lp.cls_pw, lp.fl_gamma);
             csum = warp_sum(csum);
           }
           if (lane == 0) {
@@ -159,7 +166,7 @@ __global__ void __launch_bounds__(256) loss_rows_kernel(LossPtrs P, EtbLossParam
             const float k = lp.cls_w * bs / ((float)n * (float)nc) * gs;
             for (int c = lane; c < nc; c += 32) {
               const float x = ps[5 + c];
-              atomicAdd(g + 5 + c, k * (etb_sigmoid(x) - (c == tc ? lp.cp : lp.cn)));
+              atomicAdd(g + 5 + c, k * etb_det_bce_grad(x, c == tc ? lp.cp : lp.cn, lp.cls_pw, lp.fl_gamma));
             }
           }
         }
@@ -189,7 +196,7 @@ __global__ void __launch_bounds__(256) loss_obj_fwd_kernel(LossPtrs P, EtbLossPa
   for (int64_t c = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; c < ncell; c += (int64_t)gridDim.x * blockDim.x) {
     const float t = cell_tobj(lp, S, ws, l, c);
     if (t >= 0.0f) {
-      sum += etb_bce_logits(p[c * lp.no + 4], t);
+      sum += etb_det_bce(p[c * lp.no + 4], t, lp.obj_pw, lp.fl_gamma);
       cnt += 1.0f;
     }
   }
@@ -226,7 +233,20 @@ __global__ void loss_finalize_kernel(EtbLossParams lp, LossSets S, LossWs ws, fl
         if (n3 > 0) lcls += (float)(ws.acc[l * 8 + 3] / ((double)n3 * nc));
       }
     }
-    lobj += (float)(ws.acc[l * 8 + 4] / ws.acc[l * 8 + 5]) * lp.balance[l];
+    const float obji = (float)(ws.acc[l * 8 + 4] / ws.acc[l * 8 + 5]);
+    float bal = lp.balance[l];
+    if (lp.balance_state) {
+      // autobalance (loss.py:191-193): lobj uses the balance from before the update, as a float32 scalar; the
+      // update runs in double, unfused, as Python evaluates it: b = b*0.9999 + 0.0001/obji
+      bal = (float)lp.balance_state[l];
+      ws.bal_used[l] = bal;
+      lp.balance_state[l] = __dadd_rn(__dmul_rn(lp.balance_state[l], 0.9999), __ddiv_rn(0.0001, (double)obji));
+    }
+    lobj += obji * bal;
+  }
+  if (lp.balance_state) {  // loss.py:195-196: every entry divided by the stride-16 level's
+    const double d = lp.balance_state[lp.ssi];
+    for (int l = 0; l < lp.nl; ++l) lp.balance_state[l] = __ddiv_rn(lp.balance_state[l], d);
   }
   lbox *= lp.box_w;
   lobj *= lp.obj_w;
@@ -238,7 +258,8 @@ __global__ void loss_finalize_kernel(EtbLossParams lp, LossSets S, LossWs ws, fl
 }
 
 // backward of the objectness term + dense zero-fill of every other element: one thread per element,
-// fully coalesced stores.  dL/dx4 = obj_w * B * balance_l / n_valid_l * (sigmoid(x) - tobj) for valid cells.
+// fully coalesced stores.  dL/dx4 = obj_w * B * balance_l / n_valid_l * d crit(x, tobj)/dx for valid cells
+// (crit = etb_det_bce: sigmoid(x) - tobj with the default options).
 __global__ void __launch_bounds__(256) loss_obj_bwd_kernel(LossPtrs P, EtbLossParams lp, LossSets S, LossWs ws, const float* __restrict__ gscale_dev) {
   const int l = blockIdx.y;
   const int64_t ncell = ws.cell_off[l + 1] - ws.cell_off[l];
@@ -246,14 +267,15 @@ __global__ void __launch_bounds__(256) loss_obj_bwd_kernel(LossPtrs P, EtbLossPa
   const float* __restrict__ p = P.p[l];
   float* __restrict__ g = P.g[l];
   const float gs = gscale_dev ? *gscale_dev : 1.0f;
-  const float k = lp.obj_w * (float)lp.B * lp.balance[l] / (float)ws.acc[l * 8 + 5] * gs;
+  const float bal = lp.balance_state ? ws.bal_used[l] : lp.balance[l];
+  const float k = lp.obj_w * (float)lp.B * bal / (float)ws.acc[l * 8 + 5] * gs;
   for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < nel; e += (int64_t)gridDim.x * blockDim.x) {
     const int64_t c = e / lp.no;
     const int ch = (int)(e - c * lp.no);
     float v = 0.f;
     if (ch == 4) {
       const float t = cell_tobj(lp, S, ws, l, c);
-      if (t >= 0.0f) v = k * (etb_sigmoid(p[e]) - t);
+      if (t >= 0.0f) v = k * etb_det_bce_grad(p[e], t, lp.obj_pw, lp.fl_gamma);
     }
     g[e] = v;
   }
@@ -264,6 +286,7 @@ static int loss_common(const float* const* p, const EtbLossParams* lp, const Etb
   ETB_CHECK_ARG(p && lp && sets && workspace);
   ETB_CHECK_ARG(lp->nl >= 1 && lp->nl <= ETB_MAX_LEVELS && lp->B > 0 && lp->na > 0 && lp->no > 5);
   ETB_CHECK_ARG(lp->nsets == 1 || lp->nsets == 4);
+  ETB_CHECK_ARG(lp->fl_gamma >= 0.0f && lp->ssi >= 0 && lp->ssi < lp->nl);
   ETB_CHECK_ARG(pack_sets(lp, sets, S) == 0);
   const size_t need = loss_layout(lp, sets[0].cap, (char*)workspace, ws);
   if (need > workspace_bytes) {

@@ -4,6 +4,7 @@
 //   CIoU            reference utils/metrics.py:207-249 (x1y1x2y2=False, CIoU=True, eps=1e-7)
 //   box decode      reference models/loss/loss.py:162-165   pxy = 2*sigmoid-0.5 ; pwh = (2*sigmoid)^2*anchor
 //   BCEWithLogits   torch.nn.BCEWithLogitsLoss(pos_weight=1): max(x,0) - x*z + log1p(exp(-|x|))
+//   pos_weight + FocalLoss   reference models/loss/loss.py:37-64,106-116 (etb_det_bce / etb_det_bce_grad)
 #pragma once
 #include <math.h>
 
@@ -18,6 +19,44 @@
 ETB_HD float etb_sigmoid(float x) { return 1.0f / (1.0f + expf(-x)); }
 
 ETB_HD float etb_bce_logits(float x, float z) { return fmaxf(x, 0.0f) - x * z + log1pf(expf(-fabsf(x))); }
+
+// softplus(-x) = -log(sigmoid(x))
+ETB_HD float etb_softplus_neg(float x) { return fmaxf(-x, 0.0f) + log1pf(expf(-fabsf(x))); }
+
+#define ETB_FOCAL_ALPHA 0.25f
+
+// One element of the reference's detection criterion (models/loss/loss.py:37-64, :106-116):
+//   BCEWithLogitsLoss(pos_weight=pw):  (1-z)*x + (1+(pw-1)*z)*softplus(-x)  = bce(x,z) + (pw-1)*z*softplus(-x)
+//   FocalLoss(., gamma, alpha=0.25) when gamma > 0: that times alpha_t * (1-p_t)^gamma,
+//     p_t = z*s + (1-z)*(1-s), alpha_t = z*alpha + (1-z)*(1-alpha), s = sigmoid(x).
+// The positive-weight term adds exactly +0 when pw == 1, so the defaults give etb_bce_logits bit for bit.
+ETB_HD float etb_det_bce(float x, float z, float pw, float gamma) {
+  const float b = etb_bce_logits(x, z) + (pw - 1.0f) * z * etb_softplus_neg(x);
+  if (gamma > 0.0f) {
+    const float s = etb_sigmoid(x);
+    const float pt = z * s + (1.0f - z) * (1.0f - s);
+    const float at = z * ETB_FOCAL_ALPHA + (1.0f - z) * (1.0f - ETB_FOCAL_ALPHA);
+    return b * (at * powf(1.0f - pt, gamma));
+  }
+  return b;
+}
+
+// d etb_det_bce / dx.  Weighted BCE: (1+(pw-1)z)*s - pw*z, written as (s - z) + (pw-1)*z*(s-1) (+0 when pw == 1).
+// Focal: alpha_t * (b' * m + b * gamma*(1-p_t)^(gamma-1) * (-(2z-1)*s*(1-s))), m = (1-p_t)^gamma.
+ETB_HD float etb_det_bce_grad(float x, float z, float pw, float gamma) {
+  const float s = etb_sigmoid(x);
+  const float db = (s - z) + (pw - 1.0f) * z * (s - 1.0f);
+  if (gamma > 0.0f) {
+    const float b = etb_bce_logits(x, z) + (pw - 1.0f) * z * etb_softplus_neg(x);
+    const float pt = z * s + (1.0f - z) * (1.0f - s);
+    const float at = z * ETB_FOCAL_ALPHA + (1.0f - z) * (1.0f - ETB_FOCAL_ALPHA);
+    const float q = 1.0f - pt;
+    const float m = powf(q, gamma);
+    const float dm = gamma * powf(q, gamma - 1.0f) * (-(2.0f * z - 1.0f) * s * (1.0f - s));
+    return at * (db * m + b * dm);
+  }
+  return db;
+}
 
 // CIoU of predicted box (px,py,pw,ph) vs target (tx,ty,tw,th), both centre/size.
 // If g != nullptr also returns d(ciou)/d(px,py,pw,ph) in g[0..3] (alpha treated as a constant, metrics.py:242-243).

@@ -32,7 +32,8 @@ def bbox_iou(box1, box2, x1y1x2y2=True, GIoU=False, DIoU=False, CIoU=False, eps=
 
 
 def make_loss_params(p, na, balance, box_w, obj_w, cls_w, cp, cn, nsets=1, ignore_obj=False, with_bbox=False,
-                     with_cls=False):
+                     with_cls=False, cls_pw=1.0, obj_pw=1.0, fl_gamma=0.0, balance_state=None, ssi=0):
+    """balance_state: float64 [nl] CUDA tensor (autobalance) that the forward reads and advances, or None"""
     lp = EtbLossParams()
     lp.nl = len(p)
     lp.B, lp.na, lp.no = int(p[0].shape[0]), na, int(p[0].shape[-1])
@@ -42,6 +43,8 @@ def make_loss_params(p, na, balance, box_w, obj_w, cls_w, cp, cn, nsets=1, ignor
         lp.balance[l] = float(balance[l])
     lp.box_w, lp.obj_w, lp.cls_w, lp.cp, lp.cn = float(box_w), float(obj_w), float(cls_w), float(cp), float(cn)
     lp.nsets, lp.ignore_obj, lp.with_bbox, lp.with_cls = nsets, int(ignore_obj), int(with_bbox), int(with_cls)
+    lp.cls_pw, lp.obj_pw, lp.fl_gamma, lp.ssi = float(cls_pw), float(obj_pw), float(fl_gamma), int(ssi)
+    lp.balance_state = balance_state.data_ptr() if balance_state is not None else None
     return lp
 
 
@@ -93,18 +96,28 @@ def _prep_p(p):
 
 
 class ComputeLoss:
+    """cfg.Loss.cls_pw / obj_pw (BCE positive weights), fl_gamma (focal loss) and autobalance as the reference applies
+    them (models/loss/loss.py:98-124,191-197).  With autobalance the balance lives on the device as float64 and the loss
+    kernel advances it on every call, captured replays included; `balance` reads it back (one host sync) and assigning
+    a list to it uploads in place."""
+
     def __init__(self, model, cfg):
         self.sort_obj_iou = False
-        if cfg.Loss.cls_pw != 1.0 or cfg.Loss.obj_pw != 1.0 or cfg.Loss.fl_gamma > 0 or cfg.Loss.autobalance:
-            raise NotImplementedError("fused loss supports pos_weight=1, no focal loss, no autobalance "
-                                      "(the defaults of every shipped config)")
         if cfg.Loss.assigner_type == 'SimOTA':
             raise NotImplementedError("OTA loss is not on the hot path (use_ota=False in every shipped config)")
         self.cp, self.cn = smooth_BCE(eps=cfg.Loss.label_smoothing)
+        self.cls_pw, self.obj_pw, self.fl_gamma = float(cfg.Loss.cls_pw), float(cfg.Loss.obj_pw), float(cfg.Loss.fl_gamma)
         det = model.module.head if is_parallel(model) else model.head
-        self.balance = {3: [4.0, 1.0, 0.4]}.get(det.nl, [4.0, 1.0, 0.25, 0.06, .02])
-        self.ssi = 0
-        self.gr, self.autobalance = 1.0, False
+        self.gr, self.autobalance = 1.0, bool(cfg.Loss.autobalance)
+        balance = {3: [4.0, 1.0, 0.4]}.get(det.nl, [4.0, 1.0, 0.25, 0.06, .02])
+        if self.autobalance:
+            self.ssi = [float(s) for s in det.stride].index(16.0)      # stride 16 index
+            dev = det.anchors.device
+            self.balance_state = torch.tensor(balance[:det.nl], dtype=torch.float64, device=dev)
+        else:
+            self.ssi = 0
+            self.balance_state = None
+            self._balance = balance
         nl = det.nl
         nc = 1 if cfg.single_cls else cfg.Dataset.nc
         self.box_w = cfg.Loss.box * 3.0 / nl
@@ -129,7 +142,12 @@ class ComputeLoss:
             sets = [self.assigner.assign(p, targets)]
         else:
             sets = [self.assigner.assign(p, targets, nt_dev=n_dev, cap_rows=targets.shape[0])]
-        lp = make_loss_params(p, self.na, self.balance, self.box_w, self.obj_w, self.cls_w, self.cp, self.cn)
+        if self.balance_state is not None and self.balance_state.device != p[0].device:
+            self.balance_state = self.balance_state.to(p[0].device)
+        bal = self._balance if self.balance_state is None else [0.0] * self.nl
+        lp = make_loss_params(p, self.na, bal, self.box_w, self.obj_w, self.cls_w, self.cp, self.cn,
+                              cls_pw=self.cls_pw, obj_pw=self.obj_pw, fl_gamma=self.fl_gamma,
+                              balance_state=self.balance_state, ssi=self.ssi)
         out4 = _FusedDetLoss.apply(lp, sets, "sup", *p)
         lbox, lobj, lcls = out4[0:1].detach(), out4[1:2].detach(), out4[2:3].detach()
         loss = out4[3:4]
@@ -137,3 +155,18 @@ class ComputeLoss:
 
     def __call__(self, p, targets, n_dev=None):
         return self.default_loss(p, targets, n_dev)
+
+    @property
+    def balance(self):
+        """The per-level objectness balance: a plain list, or with autobalance the device state read back as floats"""
+        if self.balance_state is None:
+            return self._balance
+        return self.balance_state.tolist()
+
+    @balance.setter
+    def balance(self, values):
+        if self.balance_state is None:
+            self._balance = list(values)
+        else:
+            with torch.no_grad():      # in place: a captured step keeps reading and advancing the same tensor
+                self.balance_state.copy_(torch.tensor(list(values), dtype=torch.float64))

@@ -14,16 +14,23 @@ from .loss import smooth_BCE, make_loss_params, _FusedDetLoss, _prep_p
 
 
 class ComputeStudentMatchLoss:
+    """cfg.Loss.cls_pw / obj_pw weight the class and objectness BCE as in the reference (ssod_loss.py:32-38); Loss.fl_gamma
+    is not read there, and Loss.autobalance only sets `ssi`, so neither changes this loss."""
+
     def __init__(self, model, cfg):
-        if cfg.Loss.cls_pw != 1.0 or cfg.Loss.obj_pw != 1.0 or cfg.Loss.autobalance or cfg.SSOD.focal_loss > 0:
-            raise NotImplementedError("fused SSOD loss supports pos_weight=1, no focal loss, no autobalance")
+        if cfg.SSOD.focal_loss > 0:
+            raise NotImplementedError("SSOD.focal_loss > 0 fails in the reference: ssod_loss.py:40-41 wraps the objectness "
+                                      "criterion in FocalLoss, which that module never imports (NameError)")
         if cfg.SSOD.use_ota:
             raise NotImplementedError("SSOD.use_ota=True is broken in the reference (SURVEY.md Appendix C #4) and "
                                       "not on the hot path")
         self.cp, self.cn = smooth_BCE(eps=cfg.Loss.label_smoothing)
+        self.cls_pw, self.obj_pw = float(cfg.Loss.cls_pw), float(cfg.Loss.obj_pw)
         det = model.module.head if is_parallel(model) else model.head
         self.balance = {3: [4.0, 1.0, 0.4]}.get(det.nl, [4.0, 1.0, 0.25, 0.06, .02])
-        self.ssi, self.gr, self.autobalance = 0, 1.0, False
+        self.autobalance = bool(cfg.Loss.autobalance)
+        self.ssi = [float(s) for s in det.stride].index(16.0) if self.autobalance else 0
+        self.gr = 1.0
         self.box_w = cfg.SSOD.box_loss_weight
         self.obj_w = cfg.SSOD.obj_loss_weight
         self.cls_w = cfg.SSOD.cls_loss_weight * cfg.Dataset.nc / 80. * 3. / det.nl
@@ -37,14 +44,13 @@ class ComputeStudentMatchLoss:
         self.pseudo_label_with_bbox = cfg.SSOD.pseudo_label_with_bbox
         self.pseudo_label_with_cls = cfg.SSOD.pseudo_label_with_cls
         self.num_keypoints = cfg.Dataset.np
-        if not self.uncertain_aug:
-            # the reference builds a single-target assigner for the *certain* set in this mode but still calls
-            # build_uc_targets_aug for the others (ssod_loss.py:205-208); only uncertain_aug=True is shipped.
-            raise NotImplementedError("SSOD.uncertain_aug=False is not on the hot path")
+        # uncertain_aug=False only asks for a single-target assigner (ssod_loss.py:65-67), whose flag the reference's
+        # assigner never reads: both settings assign identically
+        self.single_targets = not self.uncertain_aug
         for k in 'na', 'nc', 'nl', 'anchors', 'stride':
             setattr(self, k, getattr(det, k))
         self.assigner = YOLOAnchorAssigner(self.na, self.nl, self.anchors, self.anchor_t, det.stride, self.nc,
-                                           self.num_keypoints, single_targets=False, ota=False)
+                                           self.num_keypoints, single_targets=self.single_targets, ota=False)
         self._thr_cache = None
 
     def _thresholds(self, device):
@@ -91,7 +97,7 @@ class ComputeStudentMatchLoss:
             nsets = 1
         lp = make_loss_params(p, self.na, self.balance, self.box_w, self.obj_w, self.cls_w, self.cp, self.cn,
                               nsets=nsets, ignore_obj=self.ignore_obj, with_bbox=self.pseudo_label_with_bbox,
-                              with_cls=self.pseudo_label_with_cls)
+                              with_cls=self.pseudo_label_with_cls, cls_pw=self.cls_pw, obj_pw=self.obj_pw)
         out4 = _FusedDetLoss.apply(lp, sets, "ssod", *p)
         loss = out4[3:4]
         return loss, dict(ss_box=out4[0:1].detach(), ss_obj=out4[1:2].detach(), ss_cls=out4[2:3].detach())

@@ -325,7 +325,8 @@ class TrainerStep:
     def _snapshot_training_state(self):
         """The warm-up steps before a capture really train: snapshot every piece of state they touch (weights, BN
         statistics, the EMA model(s), the optimizer state -- SGD momentum, or AdamW's moments and step count --, the
-        gradients accumulated towards the next optimizer step, the training meter, the counters, lr / momentum) and return
+        gradients accumulated towards the next optimizer step, the training meter, the autobalance state of the supervised
+        loss, the counters, lr / momentum) and return
         the function that puts it back."""
         self._ensure_arena()
         emas = [e for e in (self.ema, self.semi_ema) if e is not None]
@@ -337,6 +338,8 @@ class TrainerStep:
                         for k in opt_keys if self.optimizer.state[p].get(k) is not None]
         tensors.append(self._arena.flat)     # gradients already accumulated towards the next optimizer step (accumulate > 1)
         tensors.append(self.meter.state)
+        if self.compute_loss.balance_state is not None:
+            tensors.append(self.compute_loss.balance_state)     # autobalance: every loss call advances it
         snap = [t.clone() for t in tensors]
         saved = (self.last_opt_step, [e.updates for e in emas], self.accumulate,
                  [(x['lr'], x.get('momentum')) for x in self.optimizer.param_groups])

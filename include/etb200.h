@@ -220,6 +220,12 @@ typedef struct EtbLossParams {
   int32_t ignore_obj;      /* SSOD.ignore_obj: uncertain cells -> tobj=-1 */
   int32_t with_bbox;       /* SSOD.pseudo_label_with_bbox */
   int32_t with_cls;        /* SSOD.pseudo_label_with_cls  */
+  float cls_pw, obj_pw;    /* BCEWithLogitsLoss(pos_weight=) of the class and objectness terms (1: none) */
+  float fl_gamma;          /* > 0: FocalLoss(gamma=fl_gamma, alpha=0.25) around both criteria */
+  int32_t ssi;             /* autobalance: index of the stride-16 level the balance is normalised by */
+  /* autobalance (loss.py:191-197): double[nl] balance state on the device, or NULL to use balance[] above.  When set,
+   * the forward reads it, keeps the float32 values it used for the backward, and advances it in place. */
+  double* balance_state;
 } EtbLossParams;
 
 size_t etb_loss_workspace_bytes(const EtbLossParams* lp, int32_t cap);
