@@ -123,6 +123,8 @@ _SIGS = {
     "etb_bn_partial_rows": (C.c_int32, [C.c_int64, C.c_int32, C.c_int32]),
     "etb_bn_stats": (C.c_int, [vp, C.c_int64, C.c_int32, C.c_int32, vp, C.c_int32, vp]),
     "etb_bn_finalize": (C.c_int, [vp, C.c_int32, C.c_int64, C.c_int32, vp, vp, C.c_float, C.c_float, vp, vp, vp, vp, vp, vp, vp]),
+    "etb_bn_stats_sums": (C.c_int, [vp, C.c_int64, C.c_int32, C.c_int32, vp, C.c_int32, vp, vp]),
+    "etb_bn_finalize_global": (C.c_int, [vp, C.c_int32, vp, vp, C.c_float, C.c_float, vp, vp, vp, vp, vp, vp, vp]),
     "etb_bn_act_apply_res": (C.c_int, [vp, vp, vp, vp, vp, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp]),
     "etb_maxpool5_fwd": (C.c_int, [vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp]),
     "etb_maxpool5_bwd": (C.c_int, [vp, vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp]),
@@ -132,6 +134,8 @@ _SIGS = {
     "etb_bn_act_bwd_finalize": (C.c_int, [vp, C.c_int32, C.c_int32, vp, vp, vp, C.c_int32, vp]),
     "etb_bn_act_bwd_apply": (C.c_int, [vp, vp, vp, vp, vp, vp, vp, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                        vp, vp]),
+    "etb_bn_act_bwd_apply_global": (C.c_int, [vp, vp, vp, vp, vp, vp, vp, vp, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                              C.c_int32, vp, vp]),
     "etb_nchw_f32_to_nhwc_bf16": (C.c_int, [vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                             C.c_float, vp]),
     "etb_nhwc_bf16_to_nchw_f32": (C.c_int, [vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp]),

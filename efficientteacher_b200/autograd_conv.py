@@ -443,9 +443,11 @@ class ConvBnActFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, x, weight, gamma, beta, running_mean, running_var, stride, pad, eps, momentum, act, is_stem,
-                wp=None, wd=None, res=None, dest=None, coff=0):
+                wp=None, wd=None, res=None, dest=None, coff=0, sync=None):
         """res: optional shortcut tensor added after the activation (Bottleneck, common.py:499); dest/coff: optional
-        CatBuf slice the activation is written into (the returned tensor is then that slice)."""
+        CatBuf slice the activation is written into (the returned tensor is then that slice).  sync: parallel.BnSync for
+        SyncBatchNorm (statistics of the global batch; their all-reduced vector, with the global count, is saved for the
+        backward)."""
         ctx.fan = FanIn.join(x)
         ctx.res_fan = FanIn.join(res) if res is not None else None
         ctx.has_res = res is not None
@@ -459,26 +461,28 @@ class ConvBnActFn(torch.autograd.Function):
             a = dest.slice(coff, Cout)
             ab, acs = _slice_nhwc(dest, coff, Cout)
         rb, rcs = _as_nhwc(res, Cout) if res is not None else (None, None)
-        _, stats = co.bn_forward(y, Cout, gamma.detach(), beta.detach(), running_mean, running_var, eps, momentum, act, out=ab,
-                                 out_cstride=acs, res=rb, res_cstride=rcs)
-        ctx.save_for_backward(xs, weight, y, stats)
+        r = co.bn_forward(y, Cout, gamma.detach(), beta.detach(), running_mean, running_var, eps, momentum, act, out=ab,
+                          out_cstride=acs, res=rb, res_cstride=rcs, sync=sync)
+        stats = r[1]
+        ctx.sync = sync
+        ctx.save_for_backward(xs, weight, y, stats, r[2] if sync is not None else None)
         ctx.act = act
         ctx.bn_params = (gamma, beta)        # for their .grad (gradient arena): dgamma / dbeta are accumulated in place
         return a
 
     @staticmethod
     def backward(ctx, da):
-        xs, weight, y, stats = ctx.saved_tensors
+        xs, weight, y, stats, global_sums = ctx.saved_tensors
         Cout = weight.shape[0]
         dab, dacs = _as_nhwc(da, Cout)
         gamma, beta = ctx.bn_params
         dy, dgamma, dbeta = co.bn_backward(dab, y, Cout, stats, ctx.act, da_cstride=dacs, dgamma_into=_arena_grad(gamma),
-                                           dbeta_into=_arena_grad(beta))
+                                           dbeta_into=_arena_grad(beta), sync=ctx.sync, global_sums=global_sums)
         dx, dw = _conv_backward(ctx, xs, weight, dy, Cout, ctx.fan)
         dres = None
         if ctx.has_res:
             dres = da if ctx.res_fan is None else ctx.res_fan.put(da)
-        return (dx, dw, dgamma, dbeta, None, None, None, None, None, None, None, None, None, None, dres, None, None)
+        return (dx, dw, dgamma, dbeta, None, None, None, None, None, None, None, None, None, None, dres, None, None, None)
 
 
 class DetectConvFn(torch.autograd.Function):

@@ -147,10 +147,13 @@ def conv_wgrad(x, dy, Cin, Cout, k, stride, pad, x_coffset=0, dy_coffset=0, stem
 
 
 def bn_forward(y, C_, gamma, beta, running_mean, running_var, eps, momentum, act, y_cstride=None, out=None, out_cstride=None,
-               res=None, res_cstride=None):
+               res=None, res_cstride=None, sync=None):
     """y [N,H,W,*] bf16 raw conv output -> (a bf16 same geometry, stats [4,C] fp32 = scale, shift, mean, invstd).
     `out` may be a channel slice of a wider NHWC buffer (pass its pixel stride as out_cstride); `res` (same for
-    res_cstride) is added after the activation (Bottleneck shortcut)."""
+    res_cstride) is added after the activation (Bottleneck shortcut).
+    sync (parallel.BnSync): SyncBatchNorm -- the statistics are those of the global batch (etb_bn_stats_sums, SUM
+    all-reduce of [2C+1] fp64, etb_bn_finalize_global) and the result is (a, stats, global_sums): bn_backward reads the
+    global count from global_sums on the device."""
     N, H, W, cs = y.shape
     if y_cstride is not None:
         cs = y_cstride
@@ -158,24 +161,37 @@ def bn_forward(y, C_, gamma, beta, running_mean, running_var, eps, momentum, act
     lib = _lib.lib()
     rows = int(lib.etb_bn_partial_rows(M, C_, 0))
     partials = torch.empty((rows, 2, C_), dtype=torch.float32, device=y.device)
-    _lib.check(lib.etb_bn_stats(_lib.ptr(y), M, C_, cs, _lib.ptr(partials), rows, _lib.stream_ptr()), "etb_bn_stats")
     stats = torch.empty((4, C_), dtype=torch.float32, device=y.device)
-    _lib.check(lib.etb_bn_finalize(_lib.ptr(partials), rows, M, C_, _lib.ptr(gamma), _lib.ptr(beta), float(eps), float(momentum),
-                                   _lib.ptr(running_mean), _lib.ptr(running_var), _lib.ptr(stats[0]), _lib.ptr(stats[1]),
-                                   _lib.ptr(stats[2]), _lib.ptr(stats[3]), _lib.stream_ptr()), "etb_bn_finalize")
+    st_ptrs = (_lib.ptr(stats[0]), _lib.ptr(stats[1]), _lib.ptr(stats[2]), _lib.ptr(stats[3]))
+    if sync is None:
+        _lib.check(lib.etb_bn_stats(_lib.ptr(y), M, C_, cs, _lib.ptr(partials), rows, _lib.stream_ptr()), "etb_bn_stats")
+        _lib.check(lib.etb_bn_finalize(_lib.ptr(partials), rows, M, C_, _lib.ptr(gamma), _lib.ptr(beta), float(eps), float(momentum),
+                                       _lib.ptr(running_mean), _lib.ptr(running_var), *st_ptrs, _lib.stream_ptr()), "etb_bn_finalize")
+    else:
+        sums = torch.empty(2 * C_ + 1, dtype=torch.float64, device=y.device)
+        _lib.check(lib.etb_bn_stats_sums(_lib.ptr(y), M, C_, cs, _lib.ptr(partials), rows, _lib.ptr(sums), _lib.stream_ptr()),
+                   "etb_bn_stats_sums")
+        sync.all_reduce(sums)
+        _lib.check(lib.etb_bn_finalize_global(_lib.ptr(sums), C_, _lib.ptr(gamma), _lib.ptr(beta), float(eps), float(momentum),
+                                              _lib.ptr(running_mean), _lib.ptr(running_var), *st_ptrs, _lib.stream_ptr()),
+                   "etb_bn_finalize_global")
     if out is None:
         out = nhwc_empty(N, H, W, C_, y.device)
     ocs = out.shape[3] if out_cstride is None else out_cstride
     _lib.check(lib.etb_bn_act_apply_res(_lib.ptr(y), _lib.ptr(stats[0]), _lib.ptr(stats[1]), None if res is None else _lib.ptr(res),
                                         _lib.ptr(out), M, C_, cs, 0 if res is None else (res.shape[3] if res_cstride is None else res_cstride),
                                         ocs, ACT[act], _lib.stream_ptr()), "etb_bn_act_apply_res")
-    return out, stats
+    return (out, stats) if sync is None else (out, stats, sums)
 
 
-def bn_backward(da, y, C_, stats, act, da_cstride=None, y_cstride=None, out=None, dgamma_into=None, dbeta_into=None):
+def bn_backward(da, y, C_, stats, act, da_cstride=None, y_cstride=None, out=None, dgamma_into=None, dbeta_into=None, sync=None,
+                global_sums=None):
     """da, y [N,H,W,*] bf16 -> (dy_raw bf16 [N,H,W,C], dgamma [C], dbeta [C]).  With dgamma_into / dbeta_into (the
     parameters' fp32 .grad in the gradient arena) the two sums are ADDED in place by the finalize kernel and
-    (dy, None, None) is returned -- no AccumulateGrad add kernels."""
+    (dy, None, None) is returned -- no AccumulateGrad add kernels.
+    sync / global_sums (the BnSync and the all-reduced [2C+1] of the synced forward): the sums [2C] are SUM all-reduced
+    before the apply, which divides by the global count global_sums[2C]; dgamma / dbeta stay this rank's own (torch's
+    SyncBatchNorm returns them so, and the gradient all-reduce sums them)."""
     N, H, W, ycs = y.shape
     if y_cstride is not None:
         ycs = y_cstride
@@ -195,9 +211,15 @@ def bn_backward(da, y, C_, stats, act, da_cstride=None, y_cstride=None, out=None
                "etb_bn_act_bwd_finalize")
     if out is None:
         out = nhwc_empty(N, H, W, C_, y.device)
-    _lib.check(lib.etb_bn_act_bwd_apply(_lib.ptr(da), _lib.ptr(y), _lib.ptr(stats[0]), _lib.ptr(stats[1]), _lib.ptr(stats[2]),
-                                        _lib.ptr(stats[3]), _lib.ptr(sums), M, C_, dacs, ycs, out.shape[3], ACT[act], _lib.ptr(out),
-                                        _lib.stream_ptr()), "etb_bn_act_bwd_apply")
+    if sync is None:
+        _lib.check(lib.etb_bn_act_bwd_apply(_lib.ptr(da), _lib.ptr(y), _lib.ptr(stats[0]), _lib.ptr(stats[1]), _lib.ptr(stats[2]),
+                                            _lib.ptr(stats[3]), _lib.ptr(sums), M, C_, dacs, ycs, out.shape[3], ACT[act], _lib.ptr(out),
+                                            _lib.stream_ptr()), "etb_bn_act_bwd_apply")
+    else:
+        sync.all_reduce(sums)
+        _lib.check(lib.etb_bn_act_bwd_apply_global(_lib.ptr(da), _lib.ptr(y), _lib.ptr(stats[0]), _lib.ptr(stats[1]), _lib.ptr(stats[2]),
+                                                   _lib.ptr(stats[3]), _lib.ptr(sums), _lib.ptr(global_sums), M, C_, dacs, ycs,
+                                                   out.shape[3], ACT[act], _lib.ptr(out), _lib.stream_ptr()), "etb_bn_act_bwd_apply_global")
     return (out, None, None) if acc else (out, dgb[0], dgb[1])
 
 

@@ -170,6 +170,51 @@ __global__ void __launch_bounds__(BNR_CH * BNR_GR) bn_finalize_kernel(const floa
   }
 }
 
+// ---- SyncBatchNorm, first half: one rank's statistics as ONE fp64 vector [2C+1] = sum y, sum y^2, M, ready for a SUM
+// all-reduce.  The partial rows are summed by reduce_partials with bn_finalize_kernel's block shape, so the fp32 column
+// totals are the ones etb_bn_finalize would compute; fp64 keeps the global count exact and the cross-rank sums accurate ----
+template <int BNR_CH, int BNR_GR>
+__global__ void __launch_bounds__(BNR_CH * BNR_GR) bn_sums_kernel(const float* __restrict__ partials, int nb, long M, int C,
+                                                                   double* __restrict__ sums) {
+  const int c = blockIdx.x * BNR_CH + threadIdx.x;
+  float s0 = 0.f, s1 = 0.f;
+  reduce_partials<BNR_CH, BNR_GR>(partials, nb, C, c, &s0, &s1);
+  if (threadIdx.y != 0) return;
+  if (c < C) {
+    sums[c] = (double)s0;
+    sums[C + c] = (double)s1;
+  }
+  if (blockIdx.x == 0 && threadIdx.x == 0) sums[2 * C] = (double)M;
+}
+
+// ---- SyncBatchNorm, second half: the all-reduced [2C+1] -> scale, shift, mean, invstd (etb_bn_finalize's layout) and the
+// running statistics with the global count (batch_norm_gather_stats_with_counts: momentum, unbiased var * M/(M-1)) ----
+__global__ void bn_finalize_global_kernel(const double* __restrict__ sums, int C, const float* __restrict__ gamma,
+                                          const float* __restrict__ beta, float eps, float momentum, float* __restrict__ running_mean,
+                                          float* __restrict__ running_var, float* __restrict__ scale, float* __restrict__ shift,
+                                          float* __restrict__ mean_out, float* __restrict__ invstd_out) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= C) return;
+  const double M = sums[2 * C];
+  double mean = 0.0, var = 0.0;
+  if (M > 0.0) {
+    mean = sums[c] / M;
+    var = fmax(sums[C + c] / M - mean * mean, 0.0);
+  }
+  const float meanf = (float)mean;
+  const float invstd = (float)(1.0 / sqrt(var + (double)eps));
+  const float sc = gamma[c] * invstd;
+  scale[c] = sc;
+  shift[c] = fmaf(-meanf, sc, beta[c]);
+  mean_out[c] = meanf;
+  invstd_out[c] = invstd;
+  if (running_mean && M > 0.0) {
+    const float unbiased = (float)(M > 1.0 ? var * (M / (M - 1.0)) : var);
+    running_mean[c] = fmaf(momentum, meanf - running_mean[c], running_mean[c]);
+    running_var[c] = fmaf(momentum, unbiased - running_var[c], running_var[c]);
+  }
+}
+
 // sigmoid through ONE MUFU op: s = 0.5*tanh(0.5 z) + 0.5 (tanh.approx.f32, rel. error ~2^-11: below bf16 resolution)
 __device__ __forceinline__ float tanh_approx(float x) {
   float y;
@@ -338,8 +383,9 @@ __global__ void __launch_bounds__(BN_THREADS, 2) bn_act_bwd_apply_kernel(const _
                                                                       const float* __restrict__ scale, const float* __restrict__ shift,
                                                                       const float* __restrict__ mean, const float* __restrict__ invstd,
                                                                       const float* __restrict__ sums, long M, int C, int dacs, int ycs, int ocs,
-                                                                      int act, __nv_bfloat16* __restrict__ dy) {
-  const float invM = 1.0f / (float)M;
+                                                                      int act, __nv_bfloat16* __restrict__ dy, const double* __restrict__ count) {
+  // count (SyncBatchNorm): the global count, element [2C] of the forward's all-reduced statistics; M stays the row count
+  const float invM = count ? (float)(1.0 / __ldg(count)) : 1.0f / (float)M;
   int g, lg;
   long e, stride, total;
   if (!bn_apply_index<POW2>(M, C, &g, &lg, &e, &stride, &total)) return;
@@ -477,6 +523,34 @@ extern "C" int etb_bn_finalize(const float* partials, int32_t rows, int64_t M, i
   return ETB_OK;
 }
 
+// sums [2C+1] fp64 = sum y, sum y^2, M of this rank (M == 0 allowed: zeros); partials as for etb_bn_stats (NULL when M == 0).
+// Two launches: etb_bn_stats' kernel, then the fixed-order sum of its rows.
+extern "C" int etb_bn_stats_sums(const void* y_bf16, int64_t M, int32_t C, int32_t y_cstride, float* partials, int32_t rows, double* sums,
+                                 void* stream) {
+  ETB_CHECK_ARG(sums && M >= 0 && M < (1ll << 31) && bn_c_ok(C) && y_cstride % 8 == 0 && y_cstride >= C);
+  ETB_CHECK_ARG(rows == etb_bn_partial_rows(M, C, 0) && (M == 0 || (y_bf16 && partials)));
+  if (M > 0) {
+    etb_launch(bn_stats_kernel, dim3((unsigned)rows), dim3(BN_THREADS), 0, (cudaStream_t)stream, (const __nv_bfloat16*)y_bf16, (int)M, C, y_cstride, partials);
+    ETB_CHECK_LAUNCH();
+  }
+  if (C <= 256)
+    etb_launch(bn_sums_kernel<8, 128>, dim3((C + 7) / 8), dim3(dim3(8, 128)), 0, (cudaStream_t)stream, (const float*)partials, (int)rows, (long)M, C, sums);
+  else
+    etb_launch(bn_sums_kernel<32, 32>, dim3((C + 31) / 32), dim3(dim3(32, 32)), 0, (cudaStream_t)stream, (const float*)partials, (int)rows, (long)M, C, sums);
+  ETB_CHECK_LAUNCH();
+  return ETB_OK;
+}
+
+extern "C" int etb_bn_finalize_global(const double* sums, int32_t C, const float* gamma, const float* beta, float eps, float momentum,
+                                      float* running_mean, float* running_var, float* scale, float* shift, float* mean, float* invstd,
+                                      void* stream) {
+  ETB_CHECK_ARG(sums && gamma && beta && scale && shift && mean && invstd && bn_c_ok(C) && (!running_mean == !running_var));
+  etb_launch(bn_finalize_global_kernel, dim3((C + 127) / 128), dim3(128), 0, (cudaStream_t)stream, sums, C, gamma, beta, eps, momentum,
+             running_mean, running_var, scale, shift, mean, invstd);
+  ETB_CHECK_LAUNCH();
+  return ETB_OK;
+}
+
 extern "C" int etb_bn_act_apply_res(const void* y_bf16, const float* scale, const float* shift, const void* res_bf16, void* out_bf16,
                                     int64_t M, int32_t C, int32_t y_cstride, int32_t res_cstride, int32_t out_cstride, int32_t act,
                                     void* stream) {
@@ -519,7 +593,20 @@ extern "C" int etb_bn_act_bwd_apply(const void* da_bf16, const void* y_bf16, con
   ETB_CHECK_ARG(da_bf16 && y_bf16 && scale && shift && mean && invstd && sums && dy_bf16 && M > 0 && bn_c_ok(C));
   ETB_CHECK_ARG(da_cstride % 8 == 0 && y_cstride % 8 == 0 && dy_cstride % 8 == 0 && bn_act_ok(act));
   BN_APPLY_LAUNCH(bn_act_bwd_apply_kernel, M, C, act, (cudaStream_t)stream, (const __nv_bfloat16*)da_bf16, (const __nv_bfloat16*)y_bf16, scale,
-                  shift, mean, invstd, sums, (long)M, C, da_cstride, y_cstride, dy_cstride, act, (__nv_bfloat16*)dy_bf16);
+                  shift, mean, invstd, sums, (long)M, C, da_cstride, y_cstride, dy_cstride, act, (__nv_bfloat16*)dy_bf16, (const double*)nullptr);
+  ETB_CHECK_LAUNCH();
+  return ETB_OK;
+}
+
+// SyncBatchNorm: as etb_bn_act_bwd_apply over this rank's M rows, dividing by the global count read from the device
+// (fwd_sums[2C] of the forward's all-reduced etb_bn_stats_sums vector): no host round trip, graph-safe
+extern "C" int etb_bn_act_bwd_apply_global(const void* da_bf16, const void* y_bf16, const float* scale, const float* shift, const float* mean,
+                                           const float* invstd, const float* sums, const double* fwd_sums, int64_t M, int32_t C,
+                                           int32_t da_cstride, int32_t y_cstride, int32_t dy_cstride, int32_t act, void* dy_bf16, void* stream) {
+  ETB_CHECK_ARG(da_bf16 && y_bf16 && scale && shift && mean && invstd && sums && fwd_sums && dy_bf16 && M > 0 && bn_c_ok(C));
+  ETB_CHECK_ARG(da_cstride % 8 == 0 && y_cstride % 8 == 0 && dy_cstride % 8 == 0 && bn_act_ok(act));
+  BN_APPLY_LAUNCH(bn_act_bwd_apply_kernel, M, C, act, (cudaStream_t)stream, (const __nv_bfloat16*)da_bf16, (const __nv_bfloat16*)y_bf16, scale,
+                  shift, mean, invstd, sums, (long)M, C, da_cstride, y_cstride, dy_cstride, act, (__nv_bfloat16*)dy_bf16, fwd_sums + 2 * C);
   ETB_CHECK_LAUNCH();
   return ETB_OK;
 }

@@ -19,6 +19,9 @@ import torch.nn as nn
 
 from . import _lib
 from .head import decode_levels
+from .parallel import BnSync
+
+_BN = nn.modules.batchnorm._BatchNorm      # nn.BatchNorm2d and nn.SyncBatchNorm (convert_sync_batchnorm)
 
 
 def make_divisible(x, divisor):
@@ -75,18 +78,20 @@ class Conv(nn.Module):
             self.act = nn.Identity()
         self.act_name = act if act in ("relu", "hard_swish") else None
 
-    def __deepcopy__(self, memo):   # `_packed` aliases the owning model's packer buffers: copies start without it
+    # `_packed` aliases the owning model's packer buffers and `bn_sync` holds a process group: copies start without them
+    def __deepcopy__(self, memo):
         from copy import deepcopy
         new = self.__class__.__new__(self.__class__)
         memo[id(self)] = new
         for k, v in self.__dict__.items():
-            if k != "_packed":
+            if k not in ("_packed", "bn_sync"):
                 new.__dict__[k] = deepcopy(v, memo)
         return new
 
     def __getstate__(self):
         s = dict(self.__dict__)
         s.pop("_packed", None)
+        s.pop("bn_sync", None)
         return s
 
     NATIVE = True        # training convs on the wgmma fwd/dgrad/wgrad kernels (False: torch/cuDNN scaffold)
@@ -94,6 +99,14 @@ class Conv(nn.Module):
     FUSED_GLUE = True    # concat-by-offset / fused shortcut add / native pool+upsample (csrc/glue.cu) instead of torch ops
     FUSED_FANIN = True   # gradient fan-in (C3 input, shortcut, backbone feature) accumulated in the dgrad epilogue
     is_stem = False
+    bn_sync = None       # parallel.BnSync forced on the fused BatchNorm (Model.set_bn_sync); else a SyncBatchNorm's own group
+
+    def _sync(self):
+        """The BnSync of the fused BatchNorm: the forced one, else -- for a torch.nn.SyncBatchNorm (convert_sync_batchnorm)
+        -- its process group's when torch's module would synchronise too; None: per-rank statistics."""
+        if self.bn_sync is not None:
+            return self.bn_sync
+        return BnSync.of_module(self.bn) if isinstance(self.bn, nn.SyncBatchNorm) else None
 
     def fused(self, x):
         """True when this Conv runs as ONE ConvBnActFn (and can therefore write into a CatBuf slice / add a shortcut)."""
@@ -118,7 +131,7 @@ class Conv(nn.Module):
                 bn = self.bn
                 return ConvBnActFn.apply(x, w, bn.weight, bn.bias, bn.running_mean, bn.running_var, s, p, bn.eps, bn.momentum,
                                          native_act(self.act),
-                                         self.is_stem, wp, wd, res, dest, coff)
+                                         self.is_stem, wp, wd, res, dest, coff, self._sync())
             assert dest is None
             y = self.act(self.bn(ConvFn.apply(x, w, s, p, self.is_stem, wp, wd)))
             return y if res is None else res + y
@@ -452,8 +465,24 @@ class _ModelBase(nn.Module):
         multi-tensor op; the fused BN kernels update running_mean / running_var themselves."""
         if Conv.NATIVE and Conv.FUSED_BN and self.training:
             if getattr(self, "_nbt", None) is None:
-                self._nbt = [m.num_batches_tracked for m in self.modules() if isinstance(m, nn.BatchNorm2d)]
+                self._nbt = [m.num_batches_tracked for m in self.modules() if isinstance(m, _BN)]
             torch._foreach_add_(self._nbt, 1)
+
+    def sync_batchnorm(self, process_group=None):
+        """torch.nn.SyncBatchNorm.convert_sync_batchnorm on every BatchNorm of the model, in place (the module objects that
+        hold them, their parameters and their buffers stay the same).  Training forwards then normalise with the statistics
+        of the global batch whenever torch's SyncBatchNorm would: a process group of more than one rank.  Returns self."""
+        for name, m in list(self.named_children()):
+            setattr(self, name, nn.SyncBatchNorm.convert_sync_batchnorm(m, process_group))
+        self._nbt = None
+        return self
+
+    def set_bn_sync(self, sync):
+        """Force parallel.BnSync `sync` (None: back to the default) on the fused BatchNorm of every Conv -- e.g.
+        BnSync(loopback=True), the synced kernels at world 1.  Layers on torch's BatchNorm keep their module."""
+        for m in self.modules():
+            if isinstance(m, Conv):
+                m.bn_sync = sync
 
     def engine(self):
         from .engine import TrunkEngine

@@ -4,8 +4,14 @@ student's BatchNorm running statistics before its forward.
 
 The reference wraps the student in DDP (trainer/trainer.py:313), multiplies both losses by WORLD_SIZE
 (trainer/ssod_trainer.py:638-639,647-648) and lets DDP average the bucketed gradients: mean(W*g_r) == sum(g_r).  Here the
-losses are left unscaled and the arena (GradArena) is summed once, after backward.  BatchNorm statistics stay per rank
-(SyncBN is off in every shipped config) and the teacher EMA is updated locally from the identical post-all-reduce weights.
+losses are left unscaled and the arena (GradArena) is summed once, after backward.  BatchNorm statistics stay per rank by
+default (SyncBN is off in every shipped config), and the teacher EMA is updated locally from the identical post-all-reduce
+weights.
+
+SyncBatchNorm (`sync_bn: True` with WORLD_SIZE > 1, trainer/ssod_trainer.py:217-220): the student's BatchNorm layers
+normalise with the statistics of the global batch.  BnSync is the object the fused BatchNorm kernels take for it: two SUM
+all-reduces per layer, of the forward statistics ([2C+1] fp64: sum y, sum y^2, count) and of the backward sums ([2C]
+fp32), on the current stream, over any backend (NCCL, or gloo with CUDA tensors).
 
 BatchNorm buffers (SURVEY.md 8e caveat 2): the reference's DDP runs with broadcast_buffers=True, i.e. at the start of every
 forward rank 0's running_mean / running_var overwrite every rank's.  BnBufferSync keeps all running statistics of the
@@ -67,7 +73,7 @@ class BnBufferSync:
     views of it), so DDP's per-forward `broadcast_buffers` is one collective: broadcast(src=0)."""
 
     def __init__(self, model):
-        bns = [m for m in model.modules() if isinstance(m, torch.nn.BatchNorm2d)]
+        bns = [m for m in model.modules() if isinstance(m, torch.nn.modules.batchnorm._BatchNorm)]    # SyncBatchNorm too
         n = sum(m.running_mean.numel() + m.running_var.numel() for m in bns)
         dev = bns[0].running_mean.device
         self.flat = torch.empty(n, dtype=torch.float32, device=dev)
@@ -86,3 +92,33 @@ class BnBufferSync:
         if world_size > 1:
             import torch.distributed as dist
             dist.broadcast(self.flat, src=0, group=group)
+
+
+class BnSync:
+    """The collective of the synced BatchNorm kernels (convops.bn_forward / bn_backward `sync=`): a SUM all-reduce over
+    `group` (None: the default group).  loopback=True reduces over nothing (world 1): the synced kernels and the count
+    hand-over run exactly as with several ranks, which isolates their cost from the communication."""
+
+    def __init__(self, group=None, loopback=False):
+        self.group, self.loopback = group, bool(loopback)
+        if self.loopback:
+            self.world_size = 1
+        else:
+            import torch.distributed as dist
+            self.world_size = dist.get_world_size(group)
+
+    def all_reduce(self, t):
+        if not self.loopback:
+            import torch.distributed as dist
+            dist.all_reduce(t, op=dist.ReduceOp.SUM, group=self.group)
+        return t
+
+    @classmethod
+    def of_module(cls, bn):
+        """The BnSync of a torch.nn.SyncBatchNorm module's process group, or None where torch's SyncBatchNorm would not
+        synchronise either (no initialised process group, or a group of one rank)."""
+        import torch.distributed as dist
+        if not (dist.is_available() and dist.is_initialized()):
+            return None
+        s = cls(bn.process_group)
+        return s if s.world_size > 1 else None

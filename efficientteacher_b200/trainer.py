@@ -6,10 +6,12 @@
   fwd/bwd) -> backward -> [NCCL all-reduce of the student gradients] -> SGD-Nesterov -> ema / semi-ema update
   (native fused 5-stream kernel).
 
-Data parallelism (SURVEY.md 8e): one process per GPU, per-rank batch and per-rank BN statistics exactly like the
-reference's DDP without SyncBN; the only collective is one SUM all-reduce of the flattened gradient arena per step
+Data parallelism (SURVEY.md 8e): one process per GPU, per-rank batch and, by default, per-rank BN statistics exactly like
+the reference's DDP without SyncBN; the only collective is one SUM all-reduce of the flattened gradient arena per step
 (loss*WORLD_SIZE followed by DDP's mean == sum of per-rank gradients); teachers stay bit-identical on all ranks
-because the reduced gradients are.
+because the reduced gradients are.  `sync_bn: True` with WORLD_SIZE > 1 converts the student to SyncBatchNorm like the
+reference (trainer/ssod_trainer.py:217-220, trainer/trainer.py:84-87): the eager steps then normalise with the statistics
+of the global batch (parallel.BnSync: two small all-reduces per BatchNorm layer); the captured steps refuse it.
 """
 import gc
 import math
@@ -59,6 +61,10 @@ class TrainerStep:
         self.epoch = 0
         self.batch_size = batch_size if batch_size is not None else cfg.Dataset.batch_size
         self.amp_dtype = amp_dtype
+        # the reference converts only when RANK != -1 (a single process ignores sync_bn); before the EMA is made, as there
+        self.sync_bn = bool(getattr(cfg, "sync_bn", False)) and world_size > 1
+        if self.sync_bn:
+            model.sync_batchnorm()
         self.model = model.to(device)
         self.ema = ModelEMA(self.model)          # the reference keeps it on rank 0/-1 only (trainer.py:157); harmless elsewhere
         self.semi_ema = None
@@ -91,7 +97,7 @@ class TrainerStep:
         for v in self.model.modules():
             if hasattr(v, 'bias') and isinstance(v.bias, nn.Parameter):
                 g_b.append(v.bias)
-            if isinstance(v, nn.BatchNorm2d):
+            if isinstance(v, nn.modules.batchnorm._BatchNorm):      # nn.SyncBatchNorm too
                 g_bnw.append(v.weight)
             elif hasattr(v, 'weight') and isinstance(v.weight, nn.Parameter):
                 g_w.append(v.weight)
@@ -257,6 +263,7 @@ class TrainerStep:
         scheduler) and the EMA decays of the step are host scalars written to device memory before the replay, so the
         schedule needs no re-capture.  The graphs and their buffers live in the attribute `slot`; a new key re-captures."""
         if getattr(self, slot) is None or getattr(self, slot)["key"] != key:
+            self._check_capturable()
             setattr(self, slot, None)            # release the old graphs and their memory pool before capturing new ones
             setattr(self, slot, self._capture(key, hooks, inputs, ni))
         g = getattr(self, slot)
@@ -280,6 +287,13 @@ class TrainerStep:
             g["graph_b"].replay()
             self.last_opt_step = ni
         return g["loss"]
+
+    def _check_capturable(self):
+        if self.WORLD_SIZE > 1 and any(isinstance(m, nn.SyncBatchNorm) for m in self.model.modules()):
+            raise NotImplementedError(
+                "SyncBatchNorm (sync_bn) with WORLD_SIZE > 1 runs in the eager steps only (train_instance, "
+                "train_without_unlabeled[_da], train_step): its per-layer all-reduces would have to be captured inside graph A, "
+                "and collectives inside a CUDA graph risk the NCCL teardown hazard documented in DESIGN.md section 8")
 
     def _capture(self, key, hooks, inputs, ni):
         dev = self.device
@@ -370,11 +384,13 @@ class TrainerStep:
 
 class SSODTrainerStep(TrainerStep):
     def __init__(self, cfg, device, rank=-1, world_size=1, epochs=None, batch_size=None, amp_dtype=torch.bfloat16,
-                 pseudo_label_stats=None, nb=None, start_epoch=0):
+                 pseudo_label_stats=None, nb=None, start_epoch=0, model=None):
         """pseudo_label_stats (LabelMatch only): dict(target_data_len, label_num_per_image, cls_ratio_gt) that the reference
         derives from its datasets (ssod_trainer.py:71).  nb = batches per epoch (len(train_loader)); it only sizes the
-        warm-up window exactly like trainer/trainer.py:372-376 (nb=None: the 1000-iteration floor)."""
-        super().__init__(cfg, Model(cfg), device, rank, world_size, epochs, batch_size, amp_dtype, nb, start_epoch)
+        warm-up window exactly like trainer/trainer.py:372-376 (nb=None: the 1000-iteration floor).  model: a Model(cfg)
+        built by the caller (e.g. already through convert_sync_batchnorm, the reference's order); None builds one."""
+        super().__init__(cfg, Model(cfg) if model is None else model, device, rank, world_size, epochs, batch_size, amp_dtype, nb,
+                         start_epoch)
         self.model_type = self.model.model_type
         if cfg.hyp.burn_epochs > 0:
             self.semi_ema = None
@@ -741,8 +757,10 @@ class SupTrainerStep(TrainerStep):
     and the per-iteration warm-up of lr / momentum / accumulate while ni <= nw (trainer.py:372-376, 385-395)."""
 
     def __init__(self, cfg, device, rank=-1, world_size=1, epochs=None, batch_size=None, amp_dtype=torch.bfloat16, nb=None,
-                 start_epoch=0):
-        super().__init__(cfg, SupModel(cfg), device, rank, world_size, epochs, batch_size, amp_dtype, nb, start_epoch)
+                 start_epoch=0, model=None):
+        """model: a SupModel(cfg) built by the caller (see SSODTrainerStep); None builds one."""
+        super().__init__(cfg, SupModel(cfg) if model is None else model, device, rank, world_size, epochs, batch_size, amp_dtype,
+                         nb, start_epoch)
 
     def _loss(self, imgs, targets, n_dev=None):
         if self.WORLD_SIZE > 1 and not torch.cuda.is_current_stream_capturing():

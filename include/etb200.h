@@ -306,6 +306,22 @@ int etb_bn_act_bwd_finalize(const float* partials, int32_t rows, int32_t C, floa
 int etb_bn_act_bwd_apply(const void* da_bf16, const void* y_bf16, const float* scale, const float* shift, const float* mean,
                          const float* invstd, const float* sums, int64_t M, int32_t C, int32_t da_cstride, int32_t y_cstride,
                          int32_t dy_cstride, int32_t act, void* dy_bf16, void* stream);
+/* SyncBatchNorm (torch.nn.SyncBatchNorm: statistics of the global batch across ranks).
+ *   forward : etb_bn_stats_sums (this rank's sums [2C+1] fp64 = sum y, sum y^2, M; the rows of etb_bn_stats summed in
+ *             etb_bn_finalize's fixed order; M == 0 gives zeros) -> SUM all-reduce of sums across the ranks
+ *             -> etb_bn_finalize_global (scale, shift, mean, invstd as etb_bn_finalize lays them out; running stats with the
+ *             global count: momentum, unbiased var*M/(M-1)) -> etb_bn_act_apply_res
+ *   backward: etb_bn_act_bwd_reduce -> etb_bn_act_bwd_finalize (local dgamma / dbeta, as torch's SyncBN returns them)
+ *             -> SUM all-reduce of sums[2C] -> etb_bn_act_bwd_apply_global (etb_bn_act_bwd_apply over this rank's M rows,
+ *             dividing by the global count fwd_sums[2C] of the forward's all-reduced vector, read on the device). */
+int etb_bn_stats_sums(const void* y_bf16, int64_t M, int32_t C, int32_t y_cstride, float* partials, int32_t rows, double* sums,
+                      void* stream);
+int etb_bn_finalize_global(const double* sums, int32_t C, const float* gamma, const float* beta, float eps, float momentum,
+                           float* running_mean, float* running_var, float* scale, float* shift, float* mean, float* invstd,
+                           void* stream);
+int etb_bn_act_bwd_apply_global(const void* da_bf16, const void* y_bf16, const float* scale, const float* shift, const float* mean,
+                                const float* invstd, const float* sums, const double* fwd_sums, int64_t M, int32_t C,
+                                int32_t da_cstride, int32_t y_cstride, int32_t dy_cstride, int32_t act, void* dy_bf16, void* stream);
 
 /* small layout / elementwise helpers of the trunk (all HBM-bound, coalesced 16 B vectors) */
 
