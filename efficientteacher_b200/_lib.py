@@ -6,6 +6,7 @@ compute call raises if the shared library or a CUDA device is missing.
 import ctypes as C
 import os
 
+import numpy as np
 import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -13,7 +14,7 @@ LIB_PATH = os.path.join(_HERE, "libetb200.so")
 
 ETB_MAX_LEVELS = 3
 ETB_NA = 3
-ETB_EMA_CHUNK = 4096
+ETB_CHUNK = 4096
 
 c_f32p = C.POINTER(C.c_float)
 c_i32p = C.POINTER(C.c_int32)
@@ -21,16 +22,8 @@ c_f64p = C.POINTER(C.c_double)
 vp = C.c_void_p
 
 
-class EtbEmaChunk(C.Structure):
-    _fields_ = [("v", vp), ("m", vp), ("s", vp), ("n", C.c_int32), ("pad_", C.c_int32)]
-
-
-class EtbSgdChunk(C.Structure):
-    _fields_ = [("p", vp), ("g", vp), ("buf", vp), ("n", C.c_int32), ("group", C.c_int32)]
-
-
-class EtbAdamChunk(C.Structure):
-    _fields_ = [("p", vp), ("g", vp), ("m", vp), ("v", vp), ("n", C.c_int32), ("group", C.c_int32)]
+class EtbChunk(C.Structure):
+    _fields_ = [("t", vp * 4), ("n", C.c_int32), ("group", C.c_int32)]
 
 
 class EtbNmsParams(C.Structure):
@@ -93,11 +86,7 @@ _SIGS = {
     "etb_version": (C.c_int, []),
     "etb_last_error": (C.c_char_p, []),
     "etb_launch_count": (C.c_longlong, []),
-    "etb_ema_table_count": (C.c_int64, [C.POINTER(C.c_int64), C.c_int32]),
-    "etb_ema_table_fill": (C.c_int, [C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(C.c_int64), C.c_int32,
-                                     C.POINTER(EtbEmaChunk), C.c_int64]),
-    "etb_ema_update": (C.c_int, [vp, C.c_int64, C.c_float, C.c_float, C.c_float, C.c_float, vp]),
-    "etb_ema_update_dev": (C.c_int, [vp, C.c_int64, vp, vp]),
+    "etb_ema_update": (C.c_int, [vp, C.c_int64, vp, vp]),
     "etb_sgd_step": (C.c_int, [vp, C.c_int64, vp, C.c_int32, vp]),
     "etb_adamw_step": (C.c_int, [vp, C.c_int64, vp, C.c_int32, vp]),
     "etb_detect_decode": (C.c_int, [vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
@@ -222,3 +211,39 @@ def stream_ptr(device=None):
 
 def ptr(t):
     return C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(0)
+
+
+def upload(host, device):
+    """A ctypes array or numpy array -> a uint8 tensor on `device` holding the same bytes (a descriptor table for a
+    kernel).  Not inside a stream capture: the copy from host memory would not be part of the graph."""
+    assert not torch.cuda.is_current_stream_capturing(), "descriptor table upload inside a stream capture"
+    return torch.from_numpy(np.frombuffer(host, dtype=np.uint8).copy()).to(device)
+
+
+def chunk_key(streams):
+    """The data pointers a chunk table of `streams` holds (see chunk_table); a different key means the table is stale."""
+    return tuple(t.data_ptr() if t is not None else 0 for ts in streams for t in ts)
+
+
+def chunk_table(streams, groups=None):
+    """The EtbChunk table of one multi-tensor update (etb_ema_update, etb_sgd_step, etb_adamw_step).
+
+    streams: per tensor of the list, a tuple of up to four same-size contiguous fp32 CUDA tensors in the order of the
+    kernel's EtbChunk.t (None for an unused stream); groups: per tensor, the index of its scalars in hyper_dev (default
+    0).  Returns (device table, chunk count, chunk_key(streams))."""
+    for ts in streams:
+        n = ts[0].numel()
+        if not all(t is None or (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() and t.numel() == n) for t in ts):
+            raise RuntimeError("chunk_table expects same-size contiguous fp32 CUDA tensors per entry")
+    numel = np.array([ts[0].numel() for ts in streams], dtype=np.int64)
+    ptrs = np.array([[t.data_ptr() if t is not None else 0 for t in ts] + [0] * (4 - len(ts)) for ts in streams],
+                    dtype=np.uint64).reshape(-1, 4)
+    counts = (numel + ETB_CHUNK - 1) // ETB_CHUNK
+    owner = np.repeat(np.arange(len(streams)), counts)                    # the tensor each chunk belongs to
+    start = (np.arange(len(owner)) - np.repeat(np.cumsum(counts) - counts, counts)) * ETB_CHUNK   # its first element
+    tab = np.zeros(len(owner), dtype=np.dtype(EtbChunk))
+    tab["t"] = np.where(ptrs[owner] != 0, ptrs[owner] + (4 * start).astype(np.uint64)[:, None], 0)
+    tab["n"] = np.minimum(numel[owner] - start, ETB_CHUNK)
+    tab["group"] = 0 if groups is None else np.asarray(groups, dtype=np.int32)[owner]
+    dev = next(t for t in streams[0] if t is not None).device if streams else "cuda"
+    return upload(tab, dev), len(tab), chunk_key(streams)

@@ -7,22 +7,22 @@
 // which is torch's _multi_tensor_adam (non-capturable, decoupled weight decay) op for op and rounding for rounding: each
 // foreach op rounds to fp32 once, addcmul / addcdiv are explicit fmas in ATen, and lerp's `self + w*(end - self)` is
 // contracted to an fma by torch's build.  This library builds with --fmad=false, so every fma below is written out.
-// One launch for all parameters (chunk table like the SGD one); hyper_dev[8*group + k] lives in device memory, so a
+// One launch for all parameters, one block per EtbChunk {p, g, m, v}; hyper_dev[8*group + k] lives in device memory, so a
 // captured CUDA graph of the step follows the schedule and the bias corrections of later steps.
 // HBM-bound: read p, g, m, v; write p, m, v and the zeroed g = 32 B/parameter.
 #include "common.cuh"
 
-__global__ void __launch_bounds__(256) adamw_kernel(const EtbAdamChunk* __restrict__ tab, const float* __restrict__ hyper,
+__global__ void __launch_bounds__(256) adamw_kernel(const EtbChunk* __restrict__ tab, const float* __restrict__ hyper,
                                                     int zero_grad) {
-  const EtbAdamChunk c = tab[blockIdx.x];
+  const EtbChunk c = tab[blockIdx.x];
   const float* h = hyper + 8 * c.group;
   const float decay = h[0], w1 = h[1], b2 = h[2], omb2 = h[3], step = h[4], sbc2 = h[5], eps = h[6];
   const bool small = fabsf(w1) < 0.5f;     // at::native::lerp's branch (is_lerp_weight_small)
   const float omw1 = __fsub_rn(1.f, w1);
-  float* __restrict__ p = c.p;
-  float* __restrict__ g = c.g;
-  float* __restrict__ m = c.m;
-  float* __restrict__ v = c.v;
+  float* __restrict__ p = c.t[0];
+  float* __restrict__ g = c.t[1];
+  float* __restrict__ m = c.t[2];
+  float* __restrict__ v = c.t[3];
   const int n = c.n;
   const bool vec = ((((uintptr_t)p) | ((uintptr_t)g) | ((uintptr_t)m) | ((uintptr_t)v)) & 15u) == 0;
   auto upd = [&](float& pv, float& gv, float& mv, float& vv) {
@@ -52,7 +52,7 @@ __global__ void __launch_bounds__(256) adamw_kernel(const EtbAdamChunk* __restri
   }
 }
 
-extern "C" int etb_adamw_step(const EtbAdamChunk* table_dev, int64_t n_chunks, const float* hyper_dev, int32_t zero_grad,
+extern "C" int etb_adamw_step(const EtbChunk* table_dev, int64_t n_chunks, const float* hyper_dev, int32_t zero_grad,
                               void* stream) {
   ETB_CHECK_ARG(table_dev && hyper_dev && n_chunks >= 0 && n_chunks < (1ll << 31));
   if (n_chunks == 0) return ETB_OK;

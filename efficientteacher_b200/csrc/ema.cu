@@ -10,14 +10,14 @@ __device__ __forceinline__ float ema1(float v, float m, float d, float omd) {
   return __fadd_rn(__fmul_rn(v, d), __fmul_rn(omd, m));
 }
 
-// `dev` (optional): {d, 1-d, d2, 1-d2} in device memory -- lets a captured CUDA graph replay with a new decay each step
-__global__ void __launch_bounds__(256) ema_kernel(const EtbEmaChunk* __restrict__ tab, float d, float omd, float d2, float omd2,
-                                                  const float* __restrict__ dev) {
-  if (dev) { d = dev[0]; omd = dev[1]; d2 = dev[2]; omd2 = dev[3]; }
-  const EtbEmaChunk c = tab[blockIdx.x];
-  float* __restrict__ v = c.v;
-  const float* __restrict__ m = c.m;
-  float* __restrict__ s = c.s;
+// one block per EtbChunk {v, m, s or NULL, unused}; hyper = {d, 1-d, d2, 1-d2} in device memory, so a captured CUDA
+// graph replays with the decays the host wrote there last
+__global__ void __launch_bounds__(256) ema_kernel(const EtbChunk* __restrict__ tab, const float* __restrict__ hyper) {
+  const float d = hyper[0], omd = hyper[1], d2 = hyper[2], omd2 = hyper[3];
+  const EtbChunk c = tab[blockIdx.x];
+  float* __restrict__ v = c.t[0];
+  const float* __restrict__ m = c.t[1];
+  float* __restrict__ s = c.t[2];
   const int n = c.n;
   const bool vec = ((((uintptr_t)v) | ((uintptr_t)m) | ((uintptr_t)s)) & 15u) == 0;
   if (vec) {
@@ -25,7 +25,7 @@ __global__ void __launch_bounds__(256) ema_kernel(const EtbEmaChunk* __restrict_
     float4* v4 = reinterpret_cast<float4*>(v);
     const float4* m4 = reinterpret_cast<const float4*>(m);
     float4* s4 = reinterpret_cast<float4*>(s);
-    // ETB_EMA_CHUNK/4 = 1024 float4 per chunk, 256 threads -> 4 independent 16 B loads per stream in flight
+    // ETB_CHUNK/4 = 1024 float4 per chunk, 256 threads -> 4 independent 16 B loads per stream in flight
     float4 a[4], b[4], e[4];
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
@@ -70,45 +70,10 @@ __global__ void __launch_bounds__(256) ema_kernel(const EtbEmaChunk* __restrict_
   }
 }
 
-extern "C" int64_t etb_ema_table_count(const int64_t* numel, int32_t n_tensors) {
-  int64_t c = 0;
-  for (int i = 0; i < n_tensors; ++i) c += (numel[i] + ETB_EMA_CHUNK - 1) / ETB_EMA_CHUNK;
-  return c;
-}
-
-extern "C" int etb_ema_table_fill(float* const* v, const float* const* m, float* const* s, const int64_t* numel,
-                                  int32_t n_tensors, EtbEmaChunk* out, int64_t cap) {
-  ETB_CHECK_ARG(v && m && numel && out);
-  int64_t k = 0;
-  for (int i = 0; i < n_tensors; ++i) {
-    for (int64_t o = 0; o < numel[i]; o += ETB_EMA_CHUNK) {
-      ETB_CHECK_ARG(k < cap);
-      int64_t n = numel[i] - o;
-      if (n > ETB_EMA_CHUNK) n = ETB_EMA_CHUNK;
-      out[k].v = v[i] + o;
-      out[k].m = m[i] + o;
-      out[k].s = (s && s[i]) ? s[i] + o : nullptr;
-      out[k].n = (int32_t)n;
-      out[k].pad_ = 0;
-      ++k;
-    }
-  }
-  return ETB_OK;
-}
-
-extern "C" int etb_ema_update(const EtbEmaChunk* table_dev, int64_t n_chunks, float d, float one_minus_d, float d2,
-                              float one_minus_d2, void* stream) {
-  ETB_CHECK_ARG(table_dev != nullptr && n_chunks >= 0 && n_chunks < (1ll << 31));
+extern "C" int etb_ema_update(const EtbChunk* table_dev, int64_t n_chunks, const float* hyper_dev, void* stream) {
+  ETB_CHECK_ARG(table_dev && hyper_dev && n_chunks >= 0 && n_chunks < (1ll << 31));
   if (n_chunks == 0) return ETB_OK;
-  etb_launch(ema_kernel, dim3((unsigned)n_chunks), dim3(256), 0, (cudaStream_t)stream, table_dev, d, one_minus_d, d2, one_minus_d2, nullptr);
-  ETB_CHECK_LAUNCH();
-  return ETB_OK;
-}
-
-extern "C" int etb_ema_update_dev(const EtbEmaChunk* table_dev, int64_t n_chunks, const float* scalars4_dev, void* stream) {
-  ETB_CHECK_ARG(table_dev != nullptr && scalars4_dev != nullptr && n_chunks >= 0 && n_chunks < (1ll << 31));
-  if (n_chunks == 0) return ETB_OK;
-  etb_launch(ema_kernel, dim3((unsigned)n_chunks), dim3(256), 0, (cudaStream_t)stream, table_dev, 0.f, 0.f, 0.f, 0.f, scalars4_dev);
+  etb_launch(ema_kernel, dim3((unsigned)n_chunks), dim3(256), 0, (cudaStream_t)stream, table_dev, hyper_dev);
   ETB_CHECK_LAUNCH();
   return ETB_OK;
 }

@@ -6,99 +6,131 @@ buffer exposed per parameter as state[p]['momentum_buffer'] like torch's SGD.  T
 
 FusedAdamW: the same for torch.optim.AdamW, the optimizer the reference builds when the config sets `adam: True`
 (trainer/trainer.py:211-213), on csrc/adamw.cu."""
-import ctypes as C
-
-import numpy as np
 import torch
 
 from . import _lib
-from ._lib import EtbAdamChunk, EtbSgdChunk, ETB_EMA_CHUNK
 
 
-class FusedSGD(torch.optim.Optimizer):
-    def __init__(self, params, lr=0.01, momentum=0.0, weight_decay=0.0, nesterov=True):
-        if not nesterov or momentum <= 0:
-            raise NotImplementedError("FusedSGD implements the reference's configuration: Nesterov momentum > 0")
-        super().__init__(params, dict(lr=lr, momentum=momentum, weight_decay=weight_decay, nesterov=nesterov, dampening=0))
+class _FusedOptimizer(torch.optim.Optimizer):
+    """What FusedSGD and FusedAdamW share.  Each per-parameter moment named in STATE_KEYS is a view of one flat buffer per
+    key (flat_state()), exposed as state[p][key] like torch's; the kernel KERNEL runs over the chunk table of the streams
+    {p, grad, *moments}, with the fp32 scalars of _scalars() (HYPER_W per param group) in device memory.  They are
+    uploaded only when they change, and a captured step() reads whatever refresh_hyper() wrote last."""
+    STATE_KEYS = ()
+    KERNEL = ""
+    HYPER_W = 4
+
+    def __init__(self, params, defaults):
+        super().__init__(params, defaults)
         self._table = None
         self._hyper = None
+        self._hyper_host = None
+
+    def _scalars(self):
+        raise NotImplementedError
+
+    def _next_step(self):
+        """called once per eager step() and once per refresh_hyper(), before the scalars are pushed"""
+
+    def _streams(self):
+        return [(p, p.grad) + views for (_, p), views in zip(self._ps, self._views)]
 
     def _build(self):
+        name = type(self).__name__
         ps = [(gi, p) for gi, g in enumerate(self.param_groups) for p in g["params"] if p.requires_grad]
         for _, p in ps:
             _lib.require_cuda(p)
             if p.grad is None:
-                raise RuntimeError("FusedSGD needs materialised gradients (use parallel.GradArena or run a backward first)")
+                raise RuntimeError("%s needs materialised gradients (use parallel.GradArena or run a backward first)" % name)
             if p.dtype != torch.float32 or not p.is_contiguous() or not p.grad.is_contiguous():
-                raise RuntimeError("FusedSGD expects contiguous fp32 parameters and gradients")
+                raise RuntimeError("%s expects contiguous fp32 parameters and gradients" % name)
         dev = ps[0][1].device
         total = sum(p.numel() for _, p in ps)
-        old = [self.state[p].get("momentum_buffer") for _, p in ps]
-        self._flat = torch.zeros(total, dtype=torch.float32, device=dev)
-        chunks, o = [], 0
-        for (gi, p), ob in zip(ps, old):
-            buf = self._flat[o:o + p.numel()].view_as(p)
-            if ob is not None:
-                buf.copy_(ob)
-            self.state[p]["momentum_buffer"] = buf
-            for s in range(0, p.numel(), ETB_EMA_CHUNK):
-                c = EtbSgdChunk()
-                n = min(ETB_EMA_CHUNK, p.numel() - s)
-                c.p, c.g, c.buf, c.n, c.group = p.data_ptr() + 4 * s, p.grad.data_ptr() + 4 * s, buf.data_ptr() + 4 * s, n, gi
-                chunks.append(c)
-            o += p.numel()
-        arr = (EtbSgdChunk * len(chunks))(*chunks)
-        self._table = torch.from_numpy(np.frombuffer(arr, dtype=np.uint8).copy()).to(dev)
-        self._n = len(chunks)
-        self._key = tuple((p.data_ptr(), p.grad.data_ptr()) for _, p in ps)
+        self._flat = [torch.zeros(total, dtype=torch.float32, device=dev) for _ in self.STATE_KEYS]
         self._ps = ps
-        self._hyper = torch.zeros(4 * len(self.param_groups), dtype=torch.float32, device=dev)
+        self._rehome()
+        self._table, self._n, self._key = _lib.chunk_table(self._streams(), [gi for gi, _ in ps])
+        self._hyper = torch.zeros(self.HYPER_W * len(self.param_groups), dtype=torch.float32, device=dev)
         self._hyper_host = None
 
+    @torch.no_grad()
+    def _rehome(self):
+        """Point state[p][key] at the flat buffers the kernel reads: a moment the state holds elsewhere (a new build, a
+        loaded state dict) is copied in, and a missing one is zeroed, which both torch optimizers treat as a fresh moment
+        (SGD: buf = grad on its first use; AdamW: zero moments)."""
+        self._views, missing, o = [], [], 0
+        for _, p in self._ps:
+            views = tuple(f[o:o + p.numel()].view_as(p) for f in self._flat)
+            for k, view in zip(self.STATE_KEYS, views):
+                loaded = self.state[p].get(k)
+                if loaded is None:
+                    missing.append(view)
+                elif loaded.data_ptr() != view.data_ptr():
+                    view.copy_(loaded)
+                self.state[p][k] = view
+            self._views.append(views)
+            o += p.numel()
+        if missing:
+            torch._foreach_zero_(missing)
+
+    def _ensure_table(self):
+        if self._table is None or self._key != _lib.chunk_key(self._streams()):
+            self._build()
+
     def _sync_hyper(self):
-        vals = []
-        for g in self.param_groups:
-            vals += [float(g["lr"]), float(g["momentum"]), float(g["weight_decay"]), 0.0]
-        if vals != self._hyper_host:       # H2D only when the schedule / warm-up changed something
+        vals = self._scalars()
+        if vals != self._hyper_host:       # H2D only when the step, the schedule or the warm-up changed something
             self._hyper.copy_(torch.tensor(vals, dtype=torch.float32))
             self._hyper_host = vals
+
+    def flat_state(self):
+        """The optimizer state as the flat buffers the kernel reads, one per STATE_KEYS entry (built from the current
+        parameters and gradients if no step has built them yet): restoring these restores every state[p][key]."""
+        self._ensure_table()
+        return list(self._flat)
 
     @torch.no_grad()
     def step(self, closure=None, zero_grad=True):
         if closure is not None:
             raise NotImplementedError
-        if self._table is None or self._key != tuple((p.data_ptr(), p.grad.data_ptr() if p.grad is not None else 0) for _, p in self._ps):
-            self._build()
+        self._ensure_table()
         if not torch.cuda.is_current_stream_capturing():
+            self._next_step()
             self._sync_hyper()
-        _lib.check(_lib.lib().etb_sgd_step(_lib.ptr(self._table), self._n, _lib.ptr(self._hyper), int(zero_grad), _lib.stream_ptr()),
-                   "etb_sgd_step")
+        _lib.check(getattr(_lib.lib(), self.KERNEL)(_lib.ptr(self._table), self._n, _lib.ptr(self._hyper), int(zero_grad),
+                                                    _lib.stream_ptr()), self.KERNEL)
+
+    def refresh_hyper(self):
+        """Before a replay of a captured graph that contains step(): push this step's scalars to the device memory the
+        captured kernel reads.  Call it once per replay."""
+        if self._hyper is not None:
+            self._next_step()
+            self._sync_hyper()
 
     def load_state_dict(self, state_dict):
-        """torch's load_state_dict replaces state[p]['momentum_buffer'] by fresh tensors; copy them into the flat buffer the
-        kernel reads (and keep the per-parameter views), so a resumed run really continues with the restored momentum
+        """torch's load_state_dict puts fresh tensors into the state; they are copied into the flat buffers the kernel reads
+        (the per-parameter views are kept), so a resumed run really continues with the restored moments
         (trainer/trainer.py:251: `self.optimizer.load_state_dict(ckpt['optimizer'])`)."""
         super().load_state_dict(state_dict)
         if self._table is not None:
-            with torch.no_grad():
-                o = 0
-                for _, p in self._ps:
-                    view = self._flat[o:o + p.numel()].view_as(p)
-                    loaded = self.state[p].get("momentum_buffer")
-                    if loaded is not None and loaded.data_ptr() != view.data_ptr():
-                        view.copy_(loaded)
-                    self.state[p]["momentum_buffer"] = view
-                    o += p.numel()
-        self._hyper_host = None      # force the next step to push lr / momentum / weight_decay again
-
-    def refresh_hyper(self):
-        """Push the current lr / momentum / weight_decay of the param groups to device memory (call before replaying a
-        captured graph that contains step())."""
-        if self._hyper is not None:
-            self._sync_hyper()
+            self._rehome()
+        self._hyper_host = None      # force the next step to push the scalars again
 
 
-class FusedAdamW(torch.optim.Optimizer):
+class FusedSGD(_FusedOptimizer):
+    STATE_KEYS = ("momentum_buffer",)
+    KERNEL = "etb_sgd_step"
+
+    def __init__(self, params, lr=0.01, momentum=0.0, weight_decay=0.0, nesterov=True):
+        if not nesterov or momentum <= 0:
+            raise NotImplementedError("FusedSGD implements the reference's configuration: Nesterov momentum > 0")
+        super().__init__(params, dict(lr=lr, momentum=momentum, weight_decay=weight_decay, nesterov=nesterov, dampening=0))
+
+    def _scalars(self):
+        return [v for g in self.param_groups for v in (float(g["lr"]), float(g["momentum"]), float(g["weight_decay"]), 0.0)]
+
+
+class FusedAdamW(_FusedOptimizer):
     """torch.optim.AdamW (decoupled weight decay, no amsgrad) as ONE launch over all parameters (csrc/adamw.cu), bit-equal to
     torch's default CUDA implementation (foreach) on the same gradients.  exp_avg / exp_avg_sq are views of two flat
     buffers, exposed per parameter as state[p]['exp_avg'] / state[p]['exp_avg_sq'] like torch's; the gradients are zeroed in
@@ -109,6 +141,9 @@ class FusedAdamW(torch.optim.Optimizer):
     computed in float64 on the host exactly as torch's Python does and rounded once to fp32 with the other per-group
     scalars.  It advances once per eager step(), and once per refresh_hyper(), which is called before each replay of a
     captured step(); capturing step() does not advance it.  state_dict() writes it into every state[p]['step']."""
+    STATE_KEYS = ("exp_avg", "exp_avg_sq")
+    KERNEL = "etb_adamw_step"
+    HYPER_W = 8
 
     def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=1e-2, amsgrad=False):
         if amsgrad:
@@ -117,46 +152,9 @@ class FusedAdamW(torch.optim.Optimizer):
                                       maximize=False, foreach=None, capturable=False, differentiable=False, fused=None,
                                       decoupled_weight_decay=True))
         self.step_count = 0
-        self._table = None
-        self._hyper = None
-        self._hyper_host = None
 
-    def _build(self):
-        ps = [(gi, p) for gi, g in enumerate(self.param_groups) for p in g["params"] if p.requires_grad]
-        for _, p in ps:
-            _lib.require_cuda(p)
-            if p.grad is None:
-                raise RuntimeError("FusedAdamW needs materialised gradients (use parallel.GradArena or run a backward first)")
-            if p.dtype != torch.float32 or not p.is_contiguous() or not p.grad.is_contiguous():
-                raise RuntimeError("FusedAdamW expects contiguous fp32 parameters and gradients")
-        dev = ps[0][1].device
-        total = sum(p.numel() for _, p in ps)
-        old = [(self.state[p].get("exp_avg"), self.state[p].get("exp_avg_sq")) for _, p in ps]
-        self._flat_m = torch.zeros(total, dtype=torch.float32, device=dev)
-        self._flat_v = torch.zeros(total, dtype=torch.float32, device=dev)
-        chunks, o = [], 0
-        for (gi, p), (om, ov) in zip(ps, old):
-            m = self._flat_m[o:o + p.numel()].view_as(p)
-            v = self._flat_v[o:o + p.numel()].view_as(p)
-            if om is not None:
-                m.copy_(om)
-            if ov is not None:
-                v.copy_(ov)
-            self.state[p]["exp_avg"], self.state[p]["exp_avg_sq"] = m, v
-            for s in range(0, p.numel(), ETB_EMA_CHUNK):
-                c = EtbAdamChunk()
-                c.p, c.g = p.data_ptr() + 4 * s, p.grad.data_ptr() + 4 * s
-                c.m, c.v = m.data_ptr() + 4 * s, v.data_ptr() + 4 * s
-                c.n, c.group = min(ETB_EMA_CHUNK, p.numel() - s), gi
-                chunks.append(c)
-            o += p.numel()
-        arr = (EtbAdamChunk * len(chunks))(*chunks)
-        self._table = torch.from_numpy(np.frombuffer(arr, dtype=np.uint8).copy()).to(dev)
-        self._n = len(chunks)
-        self._key = tuple((p.data_ptr(), p.grad.data_ptr()) for _, p in ps)
-        self._ps = ps
-        self._hyper = torch.zeros(8 * len(self.param_groups), dtype=torch.float32, device=dev)
-        self._hyper_host = None
+    def _next_step(self):
+        self.step_count += 1
 
     def _scalars(self):
         """Per group, the fp32 scalars of step t = step_count, each computed in float64 as torch's _multi_tensor_adam
@@ -170,31 +168,6 @@ class FusedAdamW(torch.optim.Optimizer):
             vals += [1 - lr * wd, 1 - beta1, beta2, 1 - beta2, (lr / bc1) * -1, bc2 ** 0.5, eps, 0.0]
         return vals
 
-    def _sync_hyper(self):
-        vals = self._scalars()
-        if vals != self._hyper_host:       # H2D only when the step or the schedule changed something
-            self._hyper.copy_(torch.tensor(vals, dtype=torch.float32))
-            self._hyper_host = vals
-
-    @torch.no_grad()
-    def step(self, closure=None, zero_grad=True):
-        if closure is not None:
-            raise NotImplementedError
-        if self._table is None or self._key != tuple((p.data_ptr(), p.grad.data_ptr() if p.grad is not None else 0) for _, p in self._ps):
-            self._build()
-        if not torch.cuda.is_current_stream_capturing():
-            self.step_count += 1
-            self._sync_hyper()
-        _lib.check(_lib.lib().etb_adamw_step(_lib.ptr(self._table), self._n, _lib.ptr(self._hyper), int(zero_grad),
-                                             _lib.stream_ptr()), "etb_adamw_step")
-
-    def refresh_hyper(self):
-        """Before a replay of a captured graph that contains step(): advance the step count and push this step's lr /
-        weight decay / bias corrections to the device memory the captured kernel reads.  Call it once per replay."""
-        if self._hyper is not None:
-            self.step_count += 1
-            self._sync_hyper()
-
     def _params(self):
         return [p for g in self.param_groups for p in g["params"]]
 
@@ -205,9 +178,8 @@ class FusedAdamW(torch.optim.Optimizer):
         return super().state_dict()
 
     def load_state_dict(self, state_dict):
-        """Loads torch.optim.AdamW's state dicts as well as its own (trainer/trainer.py:249-251).  The moments go into the
-        flat buffers the kernel reads (per-parameter views are kept); the per-parameter steps become step_count, so they
-        have to agree."""
+        """Loads torch.optim.AdamW's state dicts as well as its own (trainer/trainer.py:249-251).  The per-parameter steps
+        become step_count, so they have to agree."""
         super().load_state_dict(state_dict)
         ps = self._params()
         steps = [float(self.state[p].pop("step")) if "step" in self.state[p] else None for p in ps]
@@ -215,17 +187,3 @@ class FusedAdamW(torch.optim.Optimizer):
             raise ValueError("FusedAdamW keeps one step count for all parameters; the loaded state has steps %s"
                              % sorted(set(steps), key=lambda s: -1 if s is None else s))
         self.step_count = int(steps[0]) if steps and steps[0] is not None else 0
-        if self._table is not None:
-            with torch.no_grad():
-                o = 0
-                for _, p in self._ps:
-                    for k, flat in (("exp_avg", self._flat_m), ("exp_avg_sq", self._flat_v)):
-                        view = flat[o:o + p.numel()].view_as(p)
-                        loaded = self.state[p].get(k)
-                        if loaded is None:
-                            view.zero_()
-                        elif loaded.data_ptr() != view.data_ptr():
-                            view.copy_(loaded)
-                        self.state[p][k] = view
-                    o += p.numel()
-        self._hyper_host = None

@@ -5,9 +5,6 @@ must be rebuilt: forward operand [Cout][kh*kw*Cin], dgrad operand per output-par
 [Cout][128], and -- teacher only -- the folded eval-BatchNorm scale/bias.  Instead of ~3 tiny launches per conv (~440 per
 step) a WeightPacker owns persistent destination buffers and a device-resident descriptor table, and rebuilds everything
 with ONE etb_pack_multi launch (+ ONE etb_fold_bn_multi)."""
-import ctypes as C
-
-import numpy as np
 import torch
 
 from . import _lib
@@ -95,8 +92,7 @@ class WeightPacker:
                     nt = len(khs)
                     push(w, pc.dgrad.data_ptr() + 2 * off, Cin * nt * Cout, Cout, Cin, k, 3 if kind == "conv_neg" else 1, (khs, kws), ld)
                     off += Cin * nt * ld
-        darr = (EtbPackDesc * len(descs))(*descs)
-        self._descs = torch.from_numpy(np.frombuffer(darr, dtype=np.uint8).copy()).to(self.device)
+        self._descs = _lib.upload((EtbPackDesc * len(descs))(*descs), self.device)
         self._chunks = torch.tensor(chunks, dtype=torch.int32).reshape(-1, 2).contiguous().to(self.device)
         self._nchunks = len(chunks)
         self._keep = [w for w, *_ in self.items]
@@ -110,8 +106,7 @@ class WeightPacker:
                 d.mean, d.var = bn.running_mean.data_ptr(), bn.running_var.data_ptr()
                 d.scale, d.bias, d.C, d.eps = pc.scale.data_ptr(), pc.bias.data_ptr(), bn.weight.shape[0], float(bn.eps)
                 f.append(d)
-            farr = (EtbFoldDesc * len(f))(*f)
-            self._fold_descs = torch.from_numpy(np.frombuffer(farr, dtype=np.uint8).copy()).to(self.device)
+            self._fold_descs = _lib.upload((EtbFoldDesc * len(f))(*f), self.device)
             self._fold_ptrs = tuple(t.data_ptr() for bn, _ in self.folds for t in (bn.weight, bn.bias, bn.running_mean, bn.running_var))
         self._built = True
 

@@ -344,12 +344,9 @@ class TrainerStep:
         the function that puts it back."""
         self._ensure_arena()
         emas = [e for e in (self.ema, self.semi_ema) if e is not None]
-        opt_keys = ("momentum_buffer", "exp_avg", "exp_avg_sq")
-        had_momentum = any(len(self.optimizer.state[p]) for g_ in self.optimizer.param_groups for p in g_["params"])
         tensors = [t for m in [self.model] + [e.ema for e in emas] for t in m.state_dict().values()]
-        if had_momentum:
-            tensors += [self.optimizer.state[p][k] for g_ in self.optimizer.param_groups for p in g_["params"]
-                        for k in opt_keys if self.optimizer.state[p].get(k) is not None]
+        # the optimizer's moments (built here if no step has run yet: zero then, which both optimizers treat as fresh)
+        tensors += self.optimizer.flat_state()
         tensors.append(self._arena.flat)     # gradients already accumulated towards the next optimizer step (accumulate > 1)
         tensors.append(self.meter.state)
         if self.compute_loss.balance_state is not None:
@@ -363,13 +360,6 @@ class TrainerStep:
             with torch.no_grad():
                 for t, c in zip(tensors, snap):
                     t.copy_(c)
-                if not had_momentum:      # state created by the warm-up: zero == "not yet created" (SGD: buf = grad on
-                    for g_ in self.optimizer.param_groups:    # first use; AdamW: zero moments with step_count 0)
-                        for p in g_["params"]:
-                            for k in opt_keys:
-                                b = self.optimizer.state[p].get(k)
-                                if b is not None:
-                                    b.zero_()
             if step_count is not None:
                 self.optimizer.step_count = step_count
             self.last_opt_step, updates, self.accumulate, hyp = saved

@@ -41,66 +41,41 @@ const char* etb_last_error(void);
 long long etb_launch_count(void);
 
 /* ---------------------------------------------------------------------------------------------
- * EMA  (replaces the per-tensor Python loop of ModelEMA / SemiSupModelEMA / CosineEMA .update,
+ * Multi-tensor updates: the EMA, SGD and AdamW below each update every tensor of a list in ONE launch.
+ * The host splits each tensor into chunks of at most ETB_CHUNK floats and uploads one EtbChunk per chunk;
+ * the kernel runs one 256-thread block per chunk, with float4 accesses when every stream it uses is 16 B
+ * aligned.  t[] holds up to four streams, in the order each entry point documents; each block reads its
+ * per-group fp32 scalars from device memory at hyper_dev[W*group], so a captured CUDA graph replays with
+ * whatever the host wrote there last (schedule, warm-up, decays, bias corrections).
+ * ------------------------------------------------------------------------------------------- */
+typedef struct EtbChunk {
+  float* t[4];    /* the chunk's slice of each stream, NULL for an unused one */
+  int32_t n;      /* elements in this chunk (<= ETB_CHUNK) */
+  int32_t group;  /* index of the chunk's scalars in hyper_dev */
+} EtbChunk;
+#define ETB_CHUNK 4096
+
+/* EMA  (replaces the per-tensor Python loop of ModelEMA / SemiSupModelEMA / CosineEMA .update,
  *       utils/torch_utils.py:328-338, 364-375, 405-416; called from trainer/ssod_trainer.py:485-487)
- *
- * One launch updates every floating tensor of the state_dict.  The host builds a chunk table once
- * (etb_ema_table_fill), uploads it, and passes the device copy to etb_ema_update.
+ * streams {v, m, s or NULL, unused}; hyper_dev[0..3] = {d, 1-d, d2, 1-d2} (W = 4, group 0):
  *   v <- fl32(fl32(v*d) + fl32(fl32(1-d)*m))            (two roundings, no FMA: bit-exact with torch CPU)
  * and, when the chunk has a second EMA `s` (the SSOD "semi" EMA of the EMA),
- *   s <- fl32(fl32(s*d2) + fl32(fl32(1-d2)*v_new))      in the same pass (5 HBM streams instead of 6).
- * ------------------------------------------------------------------------------------------- */
-typedef struct EtbEmaChunk {
-  float* v;       /* EMA tensor slice (read+write)            */
-  const float* m; /* model tensor slice (read)                */
-  float* s;       /* optional second EMA slice, or NULL       */
-  int32_t n;      /* elements in this chunk (<= ETB_EMA_CHUNK) */
-  int32_t pad_;
-} EtbEmaChunk;
-#define ETB_EMA_CHUNK 4096
+ *   s <- fl32(fl32(s*d2) + fl32(fl32(1-d2)*v_new))      in the same pass (5 HBM streams instead of 6). */
+int etb_ema_update(const EtbChunk* table_dev, int64_t n_chunks, const float* hyper_dev, void* stream);
 
-int64_t etb_ema_table_count(const int64_t* numel, int32_t n_tensors);
-int etb_ema_table_fill(float* const* v, const float* const* m, float* const* s, const int64_t* numel,
-                       int32_t n_tensors, EtbEmaChunk* out_host, int64_t out_capacity);
-int etb_ema_update(const EtbEmaChunk* table_dev, int64_t n_chunks, float d, float one_minus_d, float d2,
-                   float one_minus_d2, void* stream);
-/* same, with {d, 1-d, d2, 1-d2} read from device memory: a captured CUDA graph of the step replays with fresh decays */
-int etb_ema_update_dev(const EtbEmaChunk* table_dev, int64_t n_chunks, const float* scalars4_dev, void* stream);
-
-/* ---------------------------------------------------------------------------------------------
- * Fused SGD-Nesterov step over all parameters (replaces torch.optim.SGD.step + zero_grad behind
+/* Fused SGD-Nesterov step over all parameters (replaces torch.optim.SGD.step + zero_grad behind
  * trainer/ssod_trainer.py:481-484; groups/hyper-parameters as built in trainer/trainer.py:193-217):
  *   g' = g + wd*p ; buf = momentum*buf + g' ; p -= lr*(g' + momentum*buf) ; (g = 0)
- * chunk table like the EMA one (<= ETB_EMA_CHUNK elements per chunk); hyper_dev[4*group + {0,1,2}] = {lr, momentum, wd}
- * lives in device memory so a captured CUDA graph follows the LR schedule.
- * ------------------------------------------------------------------------------------------- */
-typedef struct EtbSgdChunk {
-  float* p;
-  float* g;
-  float* buf;
-  int32_t n;
-  int32_t group;
-} EtbSgdChunk;
-int etb_sgd_step(const EtbSgdChunk* table_dev, int64_t n_chunks, const float* hyper_dev, int32_t zero_grad, void* stream);
+ * streams {p, g, buf, unused}; hyper_dev[4*group + {0,1,2}] = {lr, momentum, wd} (W = 4). */
+int etb_sgd_step(const EtbChunk* table_dev, int64_t n_chunks, const float* hyper_dev, int32_t zero_grad, void* stream);
 
-/* ---------------------------------------------------------------------------------------------
- * Fused AdamW step over all parameters for `adam: True` (replaces torch.optim.AdamW.step + zero_grad; optimizer built in
+/* Fused AdamW step over all parameters for `adam: True` (replaces torch.optim.AdamW.step + zero_grad; optimizer built in
  * trainer/trainer.py:211-217: AdamW(g_b, lr=lr0, betas=(momentum, 0.999)) + conv-weight and BN-weight groups), the same
  * arithmetic as torch's foreach AdamW (decoupled weight decay):
  *   p *= 1-lr*wd ; m = lerp(m, g, 1-b1) ; v = v*b2 + (1-b2)*g*g ; p += (-lr/bc1) * m / (sqrt(v)/sqrt(bc2) + eps) ; (g = 0)
- * chunk table like the SGD one (<= ETB_EMA_CHUNK elements per chunk); hyper_dev[8*group + 0..6] =
- * {1-lr*wd, 1-b1, b2, 1-b2, -lr/bc1, sqrt(bc2), eps}, computed on the host in float64 and rounded once to fp32, in
- * device memory so a captured CUDA graph follows the schedule and the bias corrections.
- * ------------------------------------------------------------------------------------------- */
-typedef struct EtbAdamChunk {
-  float* p;
-  float* g;
-  float* m;       /* exp_avg    */
-  float* v;       /* exp_avg_sq */
-  int32_t n;
-  int32_t group;
-} EtbAdamChunk;
-int etb_adamw_step(const EtbAdamChunk* table_dev, int64_t n_chunks, const float* hyper_dev, int32_t zero_grad, void* stream);
+ * streams {p, g, m = exp_avg, v = exp_avg_sq}; hyper_dev[8*group + 0..6] = {1-lr*wd, 1-b1, b2, 1-b2, -lr/bc1, sqrt(bc2),
+ * eps} (W = 8), computed on the host in float64 and rounded once to fp32. */
+int etb_adamw_step(const EtbChunk* table_dev, int64_t n_chunks, const float* hyper_dev, int32_t zero_grad, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Detect eval-mode decode (models/head/yolov5_head.py:66-78): logits [B,na,ny,nx,no] of one level ->

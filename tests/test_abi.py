@@ -38,8 +38,8 @@ def test_library_exports_all_declared_symbols(built):
     assert lib.etb_version() >= 100
 
 
-def test_struct_layouts_match_c(built, tmp_path):
-    names = ["EtbEmaChunk", "EtbNmsParams", "EtbAssignLevels", "EtbAssignOut", "EtbLossParams", "EtbFocalParams", "EtbPackDesc", "EtbFoldDesc", "EtbSgdChunk", "EtbV8Levels"]
+def test_ctypes_struct_sizes_match_c(built, tmp_path):
+    names = ["EtbChunk", "EtbNmsParams", "EtbAssignLevels", "EtbAssignOut", "EtbLossParams", "EtbFocalParams", "EtbPackDesc", "EtbFoldDesc", "EtbV8Levels"]
     if hasattr(built, "EtbConvParams") and "EtbConvParams" in open(os.path.join(ROOT, "include", "etb200.h")).read():
         names.append("EtbConvParams")
     src = '#include <stdio.h>\n#include "etb200.h"\nint main(){' + "".join(

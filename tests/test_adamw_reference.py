@@ -4,7 +4,7 @@ Trainer.build_optimizer, trainer/ssod_trainer.py:86-94 SSODTrainer.build_optimiz
 learning rate per epoch over 26 epochs of scheduler steps.  Both build_optimizer methods are called unbound on stub
 steps that hold one small module with conv, bias and BatchNorm parameters.  Runs in a subprocess (loading the reference
 patches torch process-wide); needs the reference checkout (skipped where it is absent).  Also: the ctypes mirror of
-EtbAdamChunk has the C layout."""
+EtbChunk, the chunk record of the AdamW (and SGD, EMA) kernel, has the C layout."""
 import ctypes as C
 import os
 import subprocess
@@ -97,15 +97,15 @@ def test_optimizer_and_schedule_match_reference_build_optimizer():
     assert r.returncode == 0 and "ok 12" in r.stdout, r.stdout[-4000:] + r.stderr[-4000:]
 
 
-def test_adam_chunk_layout_matches_c(tmp_path):
+def test_chunk_layout_matches_c(tmp_path):
     from efficientteacher_b200 import _lib
     src = ('#include <stdio.h>\n#include <stddef.h>\n#include "etb200.h"\nint main(){printf("%zu %zu %zu %zu\\n", '
-           'sizeof(EtbAdamChunk), offsetof(EtbAdamChunk, v), offsetof(EtbAdamChunk, n), offsetof(EtbAdamChunk, group));'
+           'sizeof(EtbChunk), offsetof(EtbChunk, t[3]), offsetof(EtbChunk, n), offsetof(EtbChunk, group));'
            'return 0;}')
     c = tmp_path / "sz.c"
     c.write_text(src)
     exe = str(tmp_path / "sz")
     subprocess.check_call(["gcc", "-I", os.path.join(ROOT, "include"), str(c), "-o", exe])
     got = [int(x) for x in subprocess.check_output([exe]).decode().split()]
-    S = _lib.EtbAdamChunk
-    assert got == [C.sizeof(S), S.v.offset, S.n.offset, S.group.offset]
+    S = _lib.EtbChunk
+    assert got == [C.sizeof(S), S.t.offset + 3 * C.sizeof(C.c_void_p), S.n.offset, S.group.offset]

@@ -21,7 +21,7 @@ def _built():
     torch.cuda.set_device(0)
 
 
-# three groups in the reference's order [bias, conv weight, BN weight]: numel % 4 != 0, numel > ETB_EMA_CHUNK (4096), and
+# three groups in the reference's order [bias, conv weight, BN weight]: numel % 4 != 0, numel > ETB_CHUNK (4096), and
 # a 1x1 1024 -> 1024 conv weight; groups 0 and 2 keep AdamW's default weight decay
 SHAPES = [[(4099,), (13,)], [(1024, 1024, 1, 1), (3, 4133)], [(77,), (513,)]]
 WD1 = 0.0005 * 32 * 2 / 64

@@ -369,6 +369,32 @@ def test_fused_sgd_load_state_dict_restores_momentum():
         assert torch.equal(a.detach(), b.detach())
 
 
+def test_fused_sgd_load_state_dict_without_momentum_starts_fresh():
+    """A torch SGD state dict saved before any step has no momentum buffers.  Loaded into a FusedSGD that has already
+    stepped, it must drop the old momentum: the next step equals torch.optim.SGD's first step (buf = grad)."""
+    from efficientteacher_b200.optim import FusedSGD
+    mk = lambda: [torch.nn.Parameter(torch.randn(s, generator=torch.Generator().manual_seed(i)).to(DEV)) for i, s in enumerate([(33,), (16, 8, 3, 3)])]  # noqa: E731
+    pa, pb = mk(), mk()
+    grads = [[torch.randn(p.shape, generator=torch.Generator().manual_seed(70 + 10 * k + i)).to(DEV) for i, p in enumerate(pa)] for k in range(2)]
+
+    def step(opt, ps, k):
+        for p, g in zip(ps, grads[k]):
+            p.grad = g.clone() if p.grad is None else p.grad.copy_(g)
+        opt.step()
+    ob = torch.optim.SGD(pb, lr=0.01, momentum=0.9, nesterov=True)
+    sd = ob.state_dict()                 # saved before any step
+    oa = FusedSGD(pa, lr=0.01, momentum=0.9, nesterov=True)
+    step(oa, pa, 0)                      # oa's flat momentum buffer now holds a history ...
+    with torch.no_grad():
+        for a, b in zip(pa, pb):
+            a.copy_(b)
+    oa.load_state_dict(sd)               # ... which the loaded state does not have
+    step(oa, pa, 1); step(ob, pb, 1)
+    for a, b in zip(pa, pb):
+        torch.testing.assert_close(a.detach(), b.detach(), rtol=2e-6, atol=1e-6)   # fma vs mul+add rounding
+        torch.testing.assert_close(oa.state[a]["momentum_buffer"], ob.state[b]["momentum_buffer"], rtol=2e-6, atol=1e-6)
+
+
 def test_labelmatch_device_path_matches_reference(golden):
     """LabelMatch on the device pipeline: rows, the per-class score lists (async pinned copy + flush) and the epoch thresholds
     against the live-reference fixture (tests/golden/labelmatch.npz)."""
