@@ -75,6 +75,11 @@ class EtbV8Levels(C.Structure):
                 ("stride", C.c_float * ETB_MAX_LEVELS)]
 
 
+class EtbLetterboxFrame(C.Structure):
+    _fields_ = [("src", vp), ("h0", C.c_int32), ("w0", C.c_int32), ("new_h", C.c_int32), ("new_w", C.c_int32), ("top", C.c_int32),
+                ("left", C.c_int32)]
+
+
 class EtbConvParams(C.Structure):
     _fields_ = [("N", C.c_int32), ("H", C.c_int32), ("W", C.c_int32), ("Cin", C.c_int32), ("Cout", C.c_int32),
                 ("kh", C.c_int32), ("kw", C.c_int32), ("stride", C.c_int32), ("pad", C.c_int32),
@@ -159,6 +164,8 @@ _SIGS = {
     "etb_pl_quality": (C.c_int, [vp, vp, C.c_int32, vp, vp, C.c_int32, vp, vp, C.c_int32, vp, C.c_int32, C.c_int32, C.c_int32,
                                  C.c_int32, vp, vp, vp, C.c_size_t, vp]),
     "etb_meter_update": (C.c_int, [vp, C.c_int32, C.POINTER(vp), C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int32, vp]),
+    "etb_letterbox_u8": (C.c_int, [vp, C.c_int32, C.c_int32, C.c_int32, vp, vp]),
+    "etb_detect_rescale": (C.c_int, [vp, vp, C.c_int32, C.c_int32, C.c_int32, vp, vp, vp]),
 }
 
 _lib = None

@@ -68,6 +68,37 @@ __global__ void __launch_bounds__(256) val_rescale_kernel(const float* __restric
   }
 }
 
+// detect.py:240, det[:, :4] = scale_coords(img.shape[2:], det[:, :4], im0.shape).round(): the rescale above, then torch.round
+// (half to even).  meta[b] = (h0, w0, inv_gain, padw, padh); out [b][d][6].
+__global__ void __launch_bounds__(256) detect_rescale_kernel(const float* __restrict__ det, const int32_t* __restrict__ det_cnt, int B,
+                                                             int max_det, int det_ld, const float* __restrict__ meta, float* __restrict__ out) {
+  const int stride = gridDim.x * blockDim.x;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < B * max_det; i += stride) {
+    const int b = i / max_det, d = i - b * max_det;
+    if (d >= det_cnt[b]) continue;
+    const float* m = meta + b * 5;
+    const float* r = det + (size_t)i * det_ld;
+    float* o = out + (size_t)i * 6;
+    o[0] = rintf(rescale_x(r[0], m[3], m[2], m[1]));
+    o[1] = rintf(rescale_x(r[1], m[4], m[2], m[0]));
+    o[2] = rintf(rescale_x(r[2], m[3], m[2], m[1]));
+    o[3] = rintf(rescale_x(r[3], m[4], m[2], m[0]));
+    o[4] = r[4];
+    o[5] = r[5];
+  }
+}
+
+extern "C" int etb_detect_rescale(const float* det, const int32_t* det_cnt, int32_t B, int32_t max_det, int32_t det_ld, const float* meta,
+                                  float* out, void* stream) {
+  ETB_CHECK_ARG(det && det_cnt && meta && out && B > 0 && max_det > 0 && det_ld >= 6);
+  const int64_t work = (int64_t)B * max_det;
+  ETB_CHECK_ARG(work < (1ll << 31));
+  const int blocks = (int)((work + 255) / 256 < 1024 ? (work + 255) / 256 : 1024);
+  etb_launch(detect_rescale_kernel, dim3(blocks), dim3(256), 0, (cudaStream_t)stream, det, det_cnt, B, max_det, det_ld, meta, out);
+  ETB_CHECK_LAUNCH();
+  return ETB_OK;
+}
+
 // One block per image: its detections go to arena rows [*arena_n + sum(det_cnt[:b]), ...).  flags[0] |= any TP bit,
 // flags[1] = 1 if the arena would overflow (those rows are dropped).
 __global__ void __launch_bounds__(256) val_append_kernel(const float* __restrict__ det_native, const int32_t* __restrict__ det_cnt,

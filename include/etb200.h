@@ -495,6 +495,30 @@ int etb_pl_quality(const double* rows, const int32_t* n_dev, int32_t n_host, con
 int etb_meter_update(double* state, int32_t cap, const void* const* src, const int32_t* slot, const int32_t* f64, int32_t n,
                      void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Batched inference (detect.py): letterbox on the device and rescale of the NMS rows to each frame.
+ *
+ * etb_letterbox_u8: frames[B] (device table) of uint8 BGR HWC source frames, each (h0, w0), resized to (new_h, new_w) and
+ * placed at (top, left) of out [B][3][H][W] uint8 RGB (the stem's uint8 input); every other pixel is 114.  The resize is
+ * cv2.resize(INTER_LINEAR) on 8UC3 bit for bit: 11-bit fixed-point coefficients, an exact integer row pass, the column pass
+ * ((((S0 >> 4) * b0) >> 16) + (((S1 >> 4) * b1) >> 16) + 2) >> 2, source columns clamped (coefficient 0) at the edges,
+ * source rows clamped without touching the coefficients, and a 2x2 box average (sum + 2) >> 2 when the frame is downscaled
+ * by exactly 2 on both axes (OpenCV's switch to INTER_AREA).  (new_h, new_w) == (h0, w0) copies.  H % 32 == W % 32 == 0 is
+ * not required, but W % 4 == 0 is.  One launch.
+ *
+ * etb_detect_rescale: det [B][max_det][det_ld>=6] fp32 NMS rows (x1,y1,x2,y2,conf,cls), det_cnt [B]; meta [B][5] fp32
+ * (h0, w0, inv_gain, padw, padh) as etb_val_epoch_append takes it -> out [B][max_det][6]: the first det_cnt[b] rows of image
+ * b in its frame's pixel space, scale_coords(...).round() as torch computes it on fp32 CUDA tensors (x - pad, times
+ * inv_gain, clamp to the frame, round half to even); other rows are not written.  One launch.
+ * ------------------------------------------------------------------------------------------- */
+typedef struct EtbLetterboxFrame {
+  const uint8_t* src;
+  int32_t h0, w0, new_h, new_w, top, left;
+} EtbLetterboxFrame;
+int etb_letterbox_u8(const EtbLetterboxFrame* frames, int32_t B, int32_t H, int32_t W, uint8_t* out, void* stream);
+int etb_detect_rescale(const float* det, const int32_t* det_cnt, int32_t B, int32_t max_det, int32_t det_ld, const float* meta,
+                       float* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
