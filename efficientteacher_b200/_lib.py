@@ -54,15 +54,20 @@ class EtbLossParams(C.Structure):
 
 class EtbPackDesc(C.Structure):
     _fields_ = [("w", vp), ("out", vp), ("elems", C.c_int64), ("Cout", C.c_int32), ("Cin", C.c_int32), ("k", C.c_int32),
-                ("mode", C.c_int32), ("ntaps", C.c_int32), ("out_ld", C.c_int32), ("kh", C.c_int8 * 12), ("kw", C.c_int8 * 12)]
+                ("mode", C.c_int32), ("ntaps", C.c_int32), ("out_ld", C.c_int32), ("dtype", C.c_int32), ("kh", C.c_int8 * 12),
+                ("kw", C.c_int8 * 12)]
 
 
 class EtbFoldDesc(C.Structure):
     _fields_ = [("gamma", vp), ("beta", vp), ("mean", vp), ("var", vp), ("scale", vp), ("bias", vp), ("C", C.c_int32),
-                ("eps", C.c_float)]
+                ("eps", C.c_float), ("dtype", C.c_int32)]
 
 
 ETB_PACK_CHUNK = 4096
+# ETB_DT_*: the element types the weight packer and the BatchNorm fold read
+ETB_DT = {torch.float32: 0, torch.float16: 1, torch.bfloat16: 2}
+# ETB_STEM_SRC_*: the image element types etb_stem_im2col_into reads
+ETB_STEM_SRC = {torch.float32: 0, torch.uint8: 1, torch.float16: 2}
 
 
 class EtbFocalParams(C.Structure):

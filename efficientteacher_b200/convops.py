@@ -252,8 +252,9 @@ def copy_slice(x, x_cstride, y, y_cstride, M, C_):
 
 # ---- the tail of the student's step (csrc/tail.cu) ----
 def stem_im2col_parts(parts, div=1.0):
-    """im2col of the stem over the batch-concatenation of `parts` ([n_i,3,H,W] uint8 or fp32 tensors) WITHOUT materialising
-    torch.cat: every part is written into its image slots of one [sum n_i, H/2, W/2, 128] buffer.  Values are x / div."""
+    """im2col of the stem over the batch-concatenation of `parts` ([n_i,3,H,W] uint8, fp32 or fp16 tensors, read as they
+    are; any other dtype goes through .float()) WITHOUT materialising torch.cat: every part is written into its image slots
+    of one [sum n_i, H/2, W/2, 128] buffer.  Values are x / div."""
     _lib.require_cuda(*parts)
     H, W = parts[0].shape[2:]
     n_tot = sum(int(p.shape[0]) for p in parts)
@@ -261,11 +262,11 @@ def stem_im2col_parts(parts, div=1.0):
     off = 0
     for p in parts:
         assert p.shape[1] == 3 and tuple(p.shape[2:]) == (H, W)
-        if p.dtype not in (torch.uint8, torch.float32):
+        if p.dtype not in _lib.ETB_STEM_SRC:
             p = p.float()
         p = p.contiguous()
         if p.shape[0]:
-            _lib.check(_lib.lib().etb_stem_im2col_into(_lib.ptr(p), int(p.dtype == torch.uint8), _lib.ptr(out), int(p.shape[0]), H, W, off,
+            _lib.check(_lib.lib().etb_stem_im2col_into(_lib.ptr(p), _lib.ETB_STEM_SRC[p.dtype], _lib.ptr(out), int(p.shape[0]), H, W, off,
                                                        float(div), _lib.stream_ptr()), "etb_stem_im2col_into")
         off += int(p.shape[0])
     return out

@@ -308,12 +308,15 @@ extern "C" int etb_domain_focal_bwd(const EtbFocalParams* fp, const float* gout,
 // of the OIHW weight row, so the weight pack is a copy.  One block = 64 consecutive output pixels of one output row: the
 // 18 (c,kh) input row segments (132 values each) are staged in shared memory with coalesced loads (zero-filled outside the
 // image = the conv padding), then every thread assembles 16 B chunks [pixel][8 k] so a warp writes 512 contiguous bytes.
-// The input is the loaders' uint8 NCHW batch (div 255) or an fp32 one (div 1); value = float(x) / div (IEEE division:
-// bit-identical to `.float() / 255`, and exact for div 1), rounded to bf16 once.  Several source batches (labeled,
-// strong-aug) are written into one im2col buffer at an image offset, which is the student's
-// torch.cat((imgs, unlabeled_imgs), 0) (ssod_trainer.py:620) without the copy.
+// The input is the loaders' uint8 NCHW batch (div 255) or an fp32 or fp16 one (div 1; val.py's `img.half() / 255`);
+// value = float(x) / div (IEEE division: bit-identical to `.float() / 255`, and exact for div 1), rounded to bf16 once.
+// Several source batches (labeled, strong-aug) are written into one im2col buffer at an image offset, which is the
+// student's torch.cat((imgs, unlabeled_imgs), 0) (ssod_trainer.py:620) without the copy.
 #define STEM_TP 64
 #define STEM_PITCH 133
+__device__ __forceinline__ float stem_f32(uint8_t v) { return (float)v; }
+__device__ __forceinline__ float stem_f32(float v) { return v; }
+__device__ __forceinline__ float stem_f32(__half v) { return __half2float(v); }   // exact: what .float() gives
 template <typename T>
 __global__ void __launch_bounds__(256) stem_im2col_any_kernel(const T* __restrict__ x, __nv_bfloat16* __restrict__ y, int N, int H, int W, float div) {
   __shared__ float sm[18 * STEM_PITCH];
@@ -329,7 +332,7 @@ __global__ void __launch_bounds__(256) stem_im2col_any_kernel(const T* __restric
     const int c = row / 6, kh = row - c * 6;
     const int ih = ih0 + kh, iw = iw0 + col;
     float v = 0.f;
-    if (ih >= 0 && ih < H && iw >= 0 && iw < W) v = __fdiv_rn((float)x[(((int64_t)n * 3 + c) * H + ih) * W + iw], div);
+    if (ih >= 0 && ih < H && iw >= 0 && iw < W) v = __fdiv_rn(stem_f32(x[(((int64_t)n * 3 + c) * H + ih) * W + iw]), div);
     sm[row * STEM_PITCH + col] = v;
   }
   __syncthreads();
@@ -356,16 +359,20 @@ __global__ void __launch_bounds__(256) stem_im2col_any_kernel(const T* __restric
   }
 }
 
-// x: [N,3,H,W] uint8 (is_u8 = 1) or fp32 (is_u8 = 0), contiguous; y: the im2col buffer [*,H/2,W/2,128] bf16 of the whole
-// (concatenated) batch; the N images of x are written starting at image index img_offset.  div: 255 for raw uint8 pixels.
-extern "C" int etb_stem_im2col_into(const void* x, int32_t is_u8, void* y_bf16, int32_t N, int32_t H, int32_t W, int32_t img_offset, float div,
+// x: [N,3,H,W] uint8 (src = ETB_STEM_SRC_U8 = 1), fp32 (ETB_STEM_SRC_F32 = 0) or fp16 (ETB_STEM_SRC_F16 = 2), contiguous;
+// y: the im2col buffer [*,H/2,W/2,128] bf16 of the whole (concatenated) batch; the N images of x are written starting at
+// image index img_offset.  div: 255 for raw uint8 pixels.
+extern "C" int etb_stem_im2col_into(const void* x, int32_t src, void* y_bf16, int32_t N, int32_t H, int32_t W, int32_t img_offset, float div,
                                     void* stream) {
   ETB_CHECK_ARG(x && y_bf16 && N > 0 && H > 0 && W > 0 && H % 2 == 0 && W % 2 == 0 && img_offset >= 0 && div > 0.f);
+  ETB_CHECK_ARG(src == ETB_STEM_SRC_F32 || src == ETB_STEM_SRC_U8 || src == ETB_STEM_SRC_F16);
   const int64_t blocks = (int64_t)N * (H / 2) * ((W / 2 + STEM_TP - 1) / STEM_TP);
   ETB_CHECK_ARG(blocks < (1ll << 31));
   __nv_bfloat16* y = (__nv_bfloat16*)y_bf16 + (size_t)img_offset * (H / 2) * (W / 2) * 128;
-  if (is_u8)
+  if (src == ETB_STEM_SRC_U8)
     etb_launch(stem_im2col_any_kernel<uint8_t>, dim3((unsigned)blocks), dim3(256), 0, (cudaStream_t)stream, (const uint8_t*)x, y, N, H, W, div);
+  else if (src == ETB_STEM_SRC_F16)
+    etb_launch(stem_im2col_any_kernel<__half>, dim3((unsigned)blocks), dim3(256), 0, (cudaStream_t)stream, (const __half*)x, y, N, H, W, div);
   else
     etb_launch(stem_im2col_any_kernel<float>, dim3((unsigned)blocks), dim3(256), 0, (cudaStream_t)stream, (const float*)x, y, N, H, W, div);
   ETB_CHECK_LAUNCH();

@@ -113,12 +113,17 @@ extern "C" int etb_upsample2x_nhwc(const void* x_bf16, void* y_bf16, int32_t N, 
 // mode 1: dgrad class  [Cin][ntaps][out_ld>=Cout] <- w[co][ci][kh_t][kw_t]   (dst: co fastest; row pitch out_ld per tap)
 // mode 2: stem [Cout][128] in the etb_stem_im2col_into K order (c,kh,kw) = the OIHW row, zero above 108
 // mode 3: mode 1 negated (dgrad operand of a conv that sits behind a GradReverse)
-__global__ void __launch_bounds__(256) pack_multi_kernel(const EtbPackDesc* __restrict__ descs, const int2* __restrict__ chunks) {
-  const int2 ch = chunks[blockIdx.x];
-  const EtbPackDesc d = descs[ch.x];
-  const float* __restrict__ w = d.w;
+// mode 4: fp32 copy of a 1-D tensor (a conv bias of a half-precision model)
+// The source is fp32, fp16 or bf16 (d.dtype, uniform per block): every value is widened to fp32 (exact) before the same
+// fp32 -> bf16 rounding, so a .half() model packs to what its fp32 copy holding the fp16 values packs to.
+__device__ __forceinline__ float to_f32(float v) { return v; }
+__device__ __forceinline__ float to_f32(__half v) { return __half2float(v); }
+__device__ __forceinline__ float to_f32(__nv_bfloat16 v) { return __bfloat162float(v); }
+
+template <typename T>
+__device__ __forceinline__ void pack_chunk(const EtbPackDesc& d, int64_t base) {
+  const T* __restrict__ w = (const T*)d.w;
   __nv_bfloat16* __restrict__ o = (__nv_bfloat16*)d.out;
-  const int64_t base = (int64_t)ch.y * ETB_PACK_CHUNK;
   const int kk = d.k * d.k;
 #pragma unroll 4
   for (int i = threadIdx.x; i < ETB_PACK_CHUNK; i += 256) {
@@ -130,22 +135,34 @@ __global__ void __launch_bounds__(256) pack_multi_kernel(const EtbPackDesc* __re
       const int ci = (int)(e % d.Cin);
       const int64_t t2 = e / d.Cin;
       const int t = (int)(t2 % kk), co = (int)(t2 / kk);
-      v = w[((int64_t)co * d.Cin + ci) * kk + t];
+      v = to_f32(w[((int64_t)co * d.Cin + ci) * kk + t]);
       if (d.out_ld > d.Cin) dst = ((int64_t)co * kk + t) * d.out_ld + ci;   // every tap padded to out_ld = ceil64(Cin) (pad stays zero)
     } else if (d.mode == 1 || d.mode == 3) {
       const int co = (int)(e % d.Cout);
       const int64_t t2 = e / d.Cout;
       const int t = (int)(t2 % d.ntaps), ci = (int)(t2 / d.ntaps);
-      v = w[(((int64_t)co * d.Cin + ci) * d.k + d.kh[t]) * d.k + d.kw[t]];
+      v = to_f32(w[(((int64_t)co * d.Cin + ci) * d.k + d.kh[t]) * d.k + d.kw[t]]);
       if (d.mode == 3) v = -v;            // GradReverse in front of the conv: dx = -(W^T dy)
       dst = ((int64_t)ci * d.ntaps + t) * d.out_ld + co;
-    } else {
+    } else if (d.mode == 2) {
       const int k = (int)(e & 127), oc = (int)(e >> 7);
       v = 0.f;
-      if (k < 108) v = w[oc * 108 + k];
+      if (k < 108) v = to_f32(w[oc * 108 + k]);
+    } else {
+      ((float*)d.out)[e] = to_f32(w[e]);
+      continue;
     }
     o[dst] = __float2bfloat16(v);
   }
+}
+
+__global__ void __launch_bounds__(256) pack_multi_kernel(const EtbPackDesc* __restrict__ descs, const int2* __restrict__ chunks) {
+  const int2 ch = chunks[blockIdx.x];
+  const EtbPackDesc d = descs[ch.x];
+  const int64_t base = (int64_t)ch.y * ETB_PACK_CHUNK;
+  if (d.dtype == ETB_DT_F16) pack_chunk<__half>(d, base);
+  else if (d.dtype == ETB_DT_BF16) pack_chunk<__nv_bfloat16>(d, base);
+  else if (d.dtype == ETB_DT_F32) pack_chunk<float>(d, base);   // any other code: nothing is read (the host refuses it)
 }
 
 extern "C" int etb_pack_multi(const EtbPackDesc* descs_dev, const void* chunks_dev, int32_t n_chunks, void* stream) {
@@ -156,13 +173,20 @@ extern "C" int etb_pack_multi(const EtbPackDesc* descs_dev, const void* chunks_d
   return ETB_OK;
 }
 
+template <typename T>
+__device__ __forceinline__ void fold_one(const EtbFoldDesc& d) {
+  const T *gamma = (const T*)d.gamma, *beta = (const T*)d.beta, *mean = (const T*)d.mean, *var = (const T*)d.var;
+  for (int c = threadIdx.x; c < d.C; c += 256) {
+    const float s = to_f32(gamma[c]) / sqrtf(to_f32(var[c]) + d.eps);
+    d.scale[c] = s;
+    d.bias[c] = to_f32(beta[c]) - to_f32(mean[c]) * s;
+  }
+}
 __global__ void __launch_bounds__(256) fold_multi_kernel(const EtbFoldDesc* __restrict__ descs) {
   const EtbFoldDesc d = descs[blockIdx.x];
-  for (int c = threadIdx.x; c < d.C; c += 256) {
-    const float s = d.gamma[c] / sqrtf(d.var[c] + d.eps);
-    d.scale[c] = s;
-    d.bias[c] = d.beta[c] - d.mean[c] * s;
-  }
+  if (d.dtype == ETB_DT_F16) fold_one<__half>(d);
+  else if (d.dtype == ETB_DT_BF16) fold_one<__nv_bfloat16>(d);
+  else if (d.dtype == ETB_DT_F32) fold_one<float>(d);
 }
 extern "C" int etb_fold_bn_multi(const EtbFoldDesc* descs_dev, int32_t n, void* stream) {
   ETB_CHECK_ARG(descs_dev && n >= 0);

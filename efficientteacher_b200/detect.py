@@ -70,7 +70,8 @@ class Predictor:
     Predictor(model)(frames) -> one [n_i, 6] fp32 CUDA tensor (x1, y1, x2, y2, conf, cls) per frame, in the frame's pixel
     space with the coordinates rounded, as detect.py's `det` after scale_coords(...).round().  frames: uint8 HWC BGR images
     (numpy arrays as cv2.imread returns them, CPU or CUDA tensors) of any sizes.  model: a Model or SupModel on a CUDA
-    device; it is put in eval() and run under no_grad on its engine (bf16 weights refreshed from its parameters each call)."""
+    device, fp32 or already .half() / .bfloat16(); it is put in eval() and run under no_grad on its engine (bf16 weights
+    refreshed from its parameters each call)."""
 
     def __init__(self, model, img_size=640, conf_thres=0.25, iou_thres=0.45, agnostic=False, max_det=1000, classes=None,
                  augment=False, half=False, num_points=0):
@@ -79,7 +80,8 @@ class Predictor:
         if augment:
             raise NotImplementedError("Predictor: augment=True (test-time augmentation) is not supported")
         if half:
-            raise NotImplementedError("Predictor: half=True is not supported (the engine computes in bf16 from fp32 weights)")
+            raise NotImplementedError("Predictor: half=True is not supported (the engine computes in bf16; a model that is "
+                                      "already .half() runs as it is)")
         if num_points or getattr(getattr(model, "head", None), "num_keypoints", 0):
             raise NotImplementedError("Predictor: keypoint heads are not supported")
         if img_size % STRIDE:

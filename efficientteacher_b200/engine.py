@@ -16,10 +16,11 @@ from .model import native_act
 
 
 class _ConvParams:
-    """Packed bf16 weights + folded BN of one Conv (refreshed from the fp32 nn.Parameters on demand)."""
+    """Packed bf16 weights + folded BN of one Conv (refreshed on demand from the nn.Parameters: fp32, or fp16 / bf16 after
+    model.half() / model.bfloat16())."""
 
-    def __init__(self, mod, stem=False):
-        self.mod, self.stem = mod, stem
+    def __init__(self, mod, stem=False, name=""):
+        self.mod, self.stem, self.name = mod, stem, name
         conv = mod.conv if hasattr(mod, "conv") else mod
         self.conv = conv
         self.bn = getattr(mod, "bn", None)
@@ -27,18 +28,24 @@ class _ConvParams:
         self.k, self.s, self.p = conv.kernel_size[0], conv.stride[0], conv.padding[0]
         self.act = native_act(getattr(mod, "act", None))
         self.w = self.scale = self.bias = None
+        self._pb = None
 
     def register(self, packer):
-        pc = packer.add(self.conv.weight, self.s, self.p, want_dgrad=False, stem=self.stem)
+        cname = self.name + ".conv" if hasattr(self.mod, "conv") else self.name
+        pc = packer.add(self.conv.weight, self.s, self.p, want_dgrad=False, stem=self.stem, name=cname + ".weight")
         self.w = pc.fwd
         if self.bn is not None:
-            packer.add_fold(self.bn, pc)
+            packer.add_fold(self.bn, pc, name=self.name + ".bn")
             self.scale, self.bias = pc.scale, pc.bias
+        elif self.conv.bias is not None:
+            self._pb = packer.add_bias(self.conv, name=cname + ".bias")
         self._pc = pc
 
     def refresh_bias(self):
+        """the epilogue reads an fp32 bias: the parameter itself, or the copy the pack launch made of an fp16 / bf16 one"""
         if self.bn is None and self.conv.bias is not None:
-            self.scale, self.bias = None, self.conv.bias.detach()
+            b = self.conv.bias.detach()
+            self.scale, self.bias = None, (b if b.dtype == torch.float32 else self._pb.fp32)
 
 
 class TrunkEngine:
@@ -48,13 +55,13 @@ class TrunkEngine:
         self.params = {}
         for name, mod in model.named_modules():
             if hasattr(mod, "conv") and hasattr(mod, "bn"):
-                self.params[name] = _ConvParams(mod, stem=(name == "backbone.stage1"))
+                self.params[name] = _ConvParams(mod, stem=(name == "backbone.stage1"), name=name)
         for i, m in enumerate(model.head.m):
-            self.params["head.m.%d" % i] = _ConvParams(m)
+            self.params["head.m.%d" % i] = _ConvParams(m, name="head.m.%d" % i)
         if self.ssod:
             for d in ("det_8", "det_16", "det_32"):
-                self.params[d + ".conv1"] = _ConvParams(getattr(model, d).conv1)
-                self.params[d + ".conv2"] = _ConvParams(getattr(model, d).conv2)
+                self.params[d + ".conv1"] = _ConvParams(getattr(model, d).conv1, name=d + ".conv1")
+                self.params[d + ".conv2"] = _ConvParams(getattr(model, d).conv2, name=d + ".conv2")
             for d in ("det_8", "det_16", "det_32"):
                 self.params[d + ".conv1"].act = "relu"
         for q in self.params.values():
@@ -65,7 +72,8 @@ class TrunkEngine:
 
     # -- helpers ------------------------------------------------------------------------------------------
     def refresh(self):
-        """Re-pack weights / re-fold BN from the current fp32 parameters (the EMA teacher changes every step)."""
+        """Re-pack weights / re-fold BN from the current parameters (the EMA teacher changes every step).  fp32, fp16 and
+        bf16 state is read as stored; any other dtype raises NotImplementedError before anything is launched."""
         if self.packer is None or self.packer.device != next(self.model.parameters()).device:
             from .packing import WeightPacker
             self.packer = WeightPacker(next(self.model.parameters()).device)
@@ -103,7 +111,8 @@ class TrunkEngine:
     # -- forward ------------------------------------------------------------------------------------------
     @torch.no_grad()
     def forward(self, x, with_features=True, refresh=True, decode=True):
-        """x [N,3,H,W] fp32 (already /255) -> ((pred [N,P,no], [raw levels]), features) like Model.forward in eval."""
+        """x [N,3,H,W] fp32 or fp16 (already /255) or uint8 -> ((pred [N,P,no], [raw levels]), features) like Model.forward
+        in eval.  The outputs are fp32 whatever the model's and the image's dtype."""
         _lib.require_cuda(x)
         m = self.model
         if refresh:
@@ -121,7 +130,8 @@ class TrunkEngine:
         cat3 = co.nhwc_empty(N, H // 16, W // 16, nk.output_p3 + ip3, dev)   # [conv3(x2), xp_2]   :102
         cat4 = co.nhwc_empty(N, H // 32, W // 32, nk.output_p4 + half5, dev)  # [conv4(x3), xp_1]   :106
         # backbone (yolov5_backbone.py:76-88)
-        # uint8 = the loaders' raw batch (value / 255 inside the im2col kernel); fp32 = the reference contract (already scaled)
+        # uint8 = the loaders' raw batch (value / 255 inside the im2col kernel); fp32 = the reference contract (already scaled);
+        # fp16 = val.py's `img.half() / 255` with a .half() model, read as stored
         col = co.stem_im2col_parts([x], 255.0 if x.dtype == torch.uint8 else 1.0)
         self.launches += 1
         x1 = self._conv("backbone.stage1", col, cin=128)

@@ -16,7 +16,7 @@ def decode_levels(levels, anchors_grid, strides):
     B, na, _, _, no = levels[0].shape
     P = sum(int(x.shape[1] * x.shape[2] * x.shape[3]) for x in levels)
     pred = torch.empty((B, P, no), dtype=torch.float32, device=levels[0].device)
-    key = (anchors_grid.data_ptr(), anchors_grid._version)
+    key = (anchors_grid.data_ptr(), anchors_grid._version, anchors_grid.dtype)   # model.half() gives the buffer new storage
     anc = _ANCHOR_CACHE.get(key)
     if anc is None:                       # one D2H per anchor tensor version, not per call (keeps the step sync-free)
         anc = _ANCHOR_CACHE[key] = anchors_grid.detach().float().cpu().contiguous()

@@ -12,6 +12,7 @@ Execution:
     torch as channels_last views.
 There is no CPU path: forward raises without a CUDA device + libetb200.so.
 """
+import itertools
 import math
 
 import torch
@@ -419,10 +420,27 @@ class _ModelBase(nn.Module):
         self.export = False
         self._engine = None
         self._packer = self._packer_aux = None
+        self._state_fp32 = None
 
     def _require(self, x):
         _lib.require_cuda(*(x if isinstance(x, (list, tuple)) else (x,)))
         _lib.lib()
+
+    def _apply(self, fn, *args, **kwargs):
+        self._state_fp32 = None       # .half() / .float() / .to(): the next forward outside the engine checks the dtypes again
+        return super()._apply(fn, *args, **kwargs)
+
+    def _require_fp32(self):
+        """The native training forward reads the parameters and the BatchNorm state as fp32 (the student trains in fp32).
+        A model after .half() / .bfloat16() runs eval() under no_grad only, on the engine; anything else raises here,
+        before a launch.  The scan runs once after every conversion (_apply), not per step."""
+        if getattr(self, "_state_fp32", None):
+            return
+        for name, t in itertools.chain(self.named_parameters(), self.named_buffers()):
+            if t.is_floating_point() and t.dtype != torch.float32:
+                raise NotImplementedError("%s is %s: the native training forward needs an fp32 model (a .half() or .bfloat16() "
+                                          "model runs in eval() under torch.no_grad())" % (name, t.dtype))
+        self._state_fp32 = True
 
     def _stem_input(self, x):
         """x: the reference's contract (one fp32 [N,3,H,W] tensor in [0,1]) or, for the native stem, a uint8 tensor / a list of
@@ -449,13 +467,15 @@ class _ModelBase(nn.Module):
         if pk is None or pk.device != dev:
             from .packing import WeightPacker
             pk = WeightPacker(dev)
-            for m in self.modules():
+            for name, m in self.named_modules():
                 if isinstance(m, Conv):
-                    m._packed = pk.add(m.conv.weight, m.conv.stride[0], m.conv.padding[0], want_dgrad=not m.is_stem, stem=m.is_stem)
-            aux = {"head": [pk.add(m.weight, 1, 0, want_dgrad=True) for m in self.head.m]}   # dgrad operand K-padded (255 -> 256)
+                    m._packed = pk.add(m.conv.weight, m.conv.stride[0], m.conv.padding[0], want_dgrad=not m.is_stem, stem=m.is_stem,
+                                       name=name + ".conv.weight")
+            aux = {"head": [pk.add(m.weight, 1, 0, want_dgrad=True, name="head.m.%d.weight" % i)      # dgrad operand K-padded (255 -> 256)
+                            for i, m in enumerate(self.head.m)]}
             for d in ("det_8", "det_16", "det_32"):      # netD.conv1 behind GradReverse: dgrad operand negated (pack mode 3)
                 if hasattr(self, d):
-                    aux[d] = pk.add(getattr(self, d).conv1.weight, 1, 0, want_dgrad=True, negate_dgrad=True)
+                    aux[d] = pk.add(getattr(self, d).conv1.weight, 1, 0, want_dgrad=True, negate_dgrad=True, name=d + ".conv1.weight")
             self._packer, self._packer_aux = pk, aux
         pk.run()
         return self._packer_aux
@@ -524,6 +544,7 @@ class Model(_ModelBase):
         self._require(x)
         if not self.training and not torch.is_grad_enabled():
             return self.engine().forward(x, with_features=True)
+        self._require_fp32()
         self._count_bn_batches()
         aux = self.pack_weights()
         f = self.neck(self.backbone(self._stem_input(x)))
@@ -545,6 +566,7 @@ class SupModel(_ModelBase):
         self._require(x)
         if not self.training and not torch.is_grad_enabled():
             return self.engine().forward(x, with_features=False)[0]
+        self._require_fp32()
         self._count_bn_batches()
         aux = self.pack_weights()
         f = self.neck(self.backbone(self._stem_input(x)))

@@ -327,29 +327,37 @@ int etb_upsample2x_bwd(const void* dy_bf16, void* dx_bf16, int32_t N, int32_t H,
                        int32_t dx_cstride, void* stream);
 int etb_copy_slice_nhwc(const void* x_bf16, void* y_bf16, int64_t M, int32_t C, int32_t x_cstride, int32_t y_cstride,
                         void* stream);
+/* element type of a packing / folding source (model.half() and model.bfloat16() state is read as stored; every value is
+ * converted to fp32 first, which is exact, so a half model packs to what its fp32 copy holding the same values packs to) */
+#define ETB_DT_F32 0
+#define ETB_DT_F16 1
+#define ETB_DT_BF16 2
 /* conv weight packing: one launch packs every conv weight of the model, or a single one (descs and the chunk list live in
- * device memory; chunk = {desc index, chunk index} covering ETB_PACK_CHUNK destination elements).  w [Cout,Cin,k,k] fp32 ->
- * bf16 K-major GEMM operands, written only at real elements (the caller zeroes the pads):
+ * device memory; chunk = {desc index, chunk index} covering ETB_PACK_CHUNK destination elements).  w [Cout,Cin,k,k] of
+ * element type dtype -> bf16 K-major GEMM operands, written only at real elements (the caller zeroes the pads):
  *   mode 0: forward operand [Cout][kh][kw][out_ld], out_ld = Cin or ceil64(Cin) (every tap padded to the 64-channel K block);
  *   mode 1: one dgrad parity class [Cin][ntaps][out_ld >= Cout] (tap t = (kh[t],kw[t]));
  *   mode 2: stem [Cout][128] in the etb_stem_im2col_into K order (c*6+kh)*6+kw = the OIHW row, zero above 108;
- *   mode 3: mode 1 with the sign flipped (dgrad operand of a conv behind GradReverse, models/detector/yolo_ssod.py:158-172). */
+ *   mode 3: mode 1 with the sign flipped (dgrad operand of a conv behind GradReverse, models/detector/yolo_ssod.py:158-172);
+ *   mode 4: out[e] = w[e] as fp32 for e < elems (the fp32 conv bias the epilogue reads, from a half-precision model). */
 #define ETB_PACK_CHUNK 4096
 typedef struct EtbPackDesc {
-  const float* w;   /* [Cout,Cin,k,k] fp32 */
-  void* out;        /* bf16 destination */
+  const void* w;    /* [Cout,Cin,k,k] of element type dtype */
+  void* out;        /* bf16 destination (mode 4: fp32) */
   int64_t elems;    /* destination elements to produce */
   int32_t Cout, Cin, k, mode, ntaps, out_ld;
+  int32_t dtype;    /* ETB_DT_* of w */
   int8_t kh[12], kw[12];
 } EtbPackDesc;
 int etb_pack_multi(const EtbPackDesc* descs_dev, const void* chunks_dev /* int32 pairs */, int32_t n_chunks, void* stream);
 typedef struct EtbFoldDesc {
-  const float *gamma, *beta, *mean, *var;
+  const void *gamma, *beta, *mean, *var;   /* [C] of element type dtype */
   float *scale, *bias;
   int32_t C;
   float eps;
+  int32_t dtype;                           /* ETB_DT_* of gamma, beta, mean and var */
 } EtbFoldDesc;
-/* eval-mode BatchNorm folded to per-channel scale/bias: scale = g/sqrt(var+eps), bias = b - mean*scale */
+/* eval-mode BatchNorm folded to per-channel scale/bias: scale = g/sqrt(var+eps), bias = b - mean*scale (in fp32) */
 int etb_fold_bn_multi(const EtbFoldDesc* descs_dev, int32_t n, void* stream);
 
 /* ---- the last library ops of the student's step (csrc/tail.cu) ----------------------------------------------------------
@@ -384,11 +392,15 @@ int64_t etb_domain_focal_workspace_bytes(void);
 int etb_domain_focal_fwd(const EtbFocalParams* fp, float* out, void* workspace, int64_t workspace_bytes, void* stream);
 int etb_domain_focal_bwd(const EtbFocalParams* fp, const float* gout, void* stream);
 /* stem im2col straight from the loaders' batch (trainer/ssod_trainer.py:694-696 `imgs.to(device).float() / 255` fused with
- * the 6x6 s2 p2 stem patch gather of models/backbone/yolov5_backbone.py:56): x is [N,3,H,W] uint8 (is_u8, div 255) or fp32
- * (div 1 for already scaled input); value = x / div (IEEE division) rounded to bf16 at K index (c*6+kh)*6+kw (the OIHW
- * weight row order) for K < 108, zeros above; the N images go to image slots [img_offset, img_offset+N) of the im2col
- * buffer y [*,H/2,W/2,128] -- torch.cat((imgs, unlabeled_imgs)) without the copy. */
-int etb_stem_im2col_into(const void* x, int32_t is_u8, void* y_bf16, int32_t N, int32_t H, int32_t W, int32_t img_offset,
+ * the 6x6 s2 p2 stem patch gather of models/backbone/yolov5_backbone.py:56): x is [N,3,H,W] of element type src, one of
+ * ETB_STEM_SRC_* (uint8 with div 255; fp32 or fp16 with div 1 for already scaled input); value = float(x) / div (IEEE
+ * division) rounded to bf16 at K index (c*6+kh)*6+kw (the OIHW weight row order) for K < 108, zeros above; the N images go
+ * to image slots [img_offset, img_offset+N) of the im2col buffer y [*,H/2,W/2,128] -- torch.cat((imgs, unlabeled_imgs))
+ * without the copy.  An fp16 batch gives what its .float() copy gives, bit for bit. */
+#define ETB_STEM_SRC_F32 0
+#define ETB_STEM_SRC_U8 1
+#define ETB_STEM_SRC_F16 2
+int etb_stem_im2col_into(const void* x, int32_t src, void* y_bf16, int32_t N, int32_t H, int32_t W, int32_t img_offset,
                          float div, void* stream);
 
 /* validation matching (val.py:123-145 process_batch), all images of a batch in one launch: correct[b][d][i] = detection d of
