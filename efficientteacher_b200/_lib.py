@@ -157,6 +157,11 @@ _SIGS = {
     "etb_val_epoch_append_workspace_bytes": (C.c_size_t, [C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
     "etb_val_epoch_append": (C.c_int, [vp, vp, C.c_int32, C.c_int32, C.c_int32, vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                        vp, C.c_int32, C.c_int32, vp, vp, vp, C.c_int64, vp, vp, vp, vp, C.c_size_t, vp]),
+    "etb_val_epoch_append_confusion": (C.c_int, [vp, vp, C.c_int32, C.c_int32, C.c_int32, vp, vp, C.c_int32, C.c_int32, C.c_int32,
+                                                 C.c_int32, vp, C.c_int32, C.c_int32, vp, vp, vp, C.c_int64, vp, vp, vp, C.c_int32,
+                                                 C.c_float, C.c_float, vp, vp, vp, C.c_size_t, vp]),
+    "etb_confusion_matrix": (C.c_int, [vp, vp, C.c_int32, C.c_int32, C.c_int32, vp, C.c_int32, C.c_int32, C.c_float, C.c_float, vp, vp,
+                                       vp]),
     "etb_ap_per_class_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int32]),
     "etb_ap_per_class": (C.c_int, [vp, vp, vp, C.c_int64, C.c_int32, vp, C.c_int32, C.c_int32, vp, vp, vp, vp, vp, vp, vp, vp,
                                    C.c_size_t, vp]),

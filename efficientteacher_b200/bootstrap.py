@@ -17,6 +17,7 @@ Modules of the host application imported later with `from X import Y` see the pa
 import importlib
 import inspect
 import sys
+import types
 
 from . import _lib, ema, labelmatch, loss, metrics, model, nms, pl_quality, pseudo_label, ssod_loss, assigner, tal
 from . import val as etb_val
@@ -78,6 +79,23 @@ def _ap_per_class(original):
     return ap_per_class
 
 
+def _confusion_matrix(original):
+    """utils.metrics.ConfusionMatrix (metrics.py:129-204), also val.py's by-name binding: the native class
+    (efficientteacher_b200.metrics), whose process_batch runs on the device for CUDA tensors; calls with a CPU tensor run the
+    host application's own process_batch into a host-side matrix that `matrix` adds in.  plot is the original plot, which
+    reads only self.matrix and self.nc."""
+    class ConfusionMatrix(metrics.ConfusionMatrix):
+        host_plot = original.plot
+
+        def process_batch(self, detections, labels):
+            if detections.is_cuda and labels.is_cuda:
+                return super().process_batch(detections, labels)
+            host = types.SimpleNamespace(matrix=self.host, nc=self.nc, conf=self.conf, iou_thres=self.iou_thres)
+            return original.process_batch(host, detections, labels)
+    ConfusionMatrix.__wrapped__ = original
+    return ConfusionMatrix
+
+
 # (defining module, attribute, replacement | factory(original) -> replacement)
 _PATCHES = [
     ("utils.torch_utils", "ModelEMA", ema.ModelEMA),
@@ -87,6 +105,7 @@ _PATCHES = [
     ("utils.general", "non_max_suppression", _val_nms),
     ("utils.metrics", "bbox_iou", _bbox_iou),
     ("utils.metrics", "ap_per_class", _ap_per_class),
+    ("utils.metrics", "ConfusionMatrix", _confusion_matrix),
     ("val", "run", _val_run),
     ("utils.self_supervised_utils", "FairPseudoLabel", pseudo_label.FairPseudoLabel),
     ("utils.self_supervised_utils", "check_pseudo_label_with_gt", pl_quality.check_pseudo_label_with_gt),   # ssod_trainer.py:46
@@ -99,7 +118,7 @@ _PATCHES = [
     ("models.detector.yolo_ssod", "Model", model.Model),
     ("models.detector.yolo", "Model", model.SupModel),
 ]
-_FACTORIES = (_val_nms, _bbox_iou, _ap_per_class, _val_run)
+_FACTORIES = (_val_nms, _bbox_iou, _ap_per_class, _confusion_matrix, _val_run)
 # defining modules whose import may fail (val.py pulls in optional dependencies of the host application): their patches are
 # skipped, listed in apply.skipped
 _OPTIONAL = ("val",)

@@ -4,7 +4,8 @@
 //   the NMS rows of every image are rescaled to its native image space (utils/general.py scale_coords with the loader's
 //   ratio_pad), the normalised xywh targets become native-space xyxy labels, etb_val_process_batch matches them, and each
 //   detection's (conf, class, correct bits) is appended to an epoch arena at a running offset kept in device memory.
-//   The label classes go into an int32 histogram (etb_label_class_hist).
+//   The label classes go into an int32 histogram (etb_label_class_hist).  etb_val_epoch_append_confusion also adds the
+//   rescaled rows and labels into a confusion matrix (etb_confusion_matrix, csrc/val.cu).
 // Epoch end (etb_ap_per_class): the numeric core of ap_per_class -- sort by (class, conf descending), segmented cumulative
 //   TP / FP counts, precision / recall in float64, the precision envelope, numpy.interp at the 101 COCO recall points of
 //   compute_ap and at the 1000 confidence points of the P and R curves.  The O(nc * 1000) tail (trapz, F1, argmax, means)
@@ -143,11 +144,19 @@ extern "C" size_t etb_val_epoch_append_workspace_bytes(int32_t B, int32_t max_de
          align256((size_t)B * max_det * T);
 }
 
-extern "C" int etb_val_epoch_append(const float* det, const int32_t* det_cnt, int32_t B, int32_t max_det, int32_t det_ld,
-                                    const float* img_meta, const float* targets, int32_t nt, int32_t H, int32_t W, int32_t single_cls,
-                                    const float* iouv, int32_t T, int32_t nc, float* arena_conf, float* arena_cls, uint16_t* arena_tp,
-                                    int64_t arena_cap, int64_t* arena_n, int32_t* hist, int32_t* flags, void* workspace,
-                                    size_t workspace_bytes, void* stream) {
+// The confusion matrix a batch is also added into (etb_val_epoch_append_confusion); NULL: none.
+struct ConfusionArgs {
+  int32_t nc;
+  float conf_thres, iou_thres;
+  int64_t* matrix;
+  int32_t* flags;
+};
+
+static int val_epoch_append(const float* det, const int32_t* det_cnt, int32_t B, int32_t max_det, int32_t det_ld, const float* img_meta,
+                            const float* targets, int32_t nt, int32_t H, int32_t W, int32_t single_cls, const float* iouv, int32_t T,
+                            int32_t nc, float* arena_conf, float* arena_cls, uint16_t* arena_tp, int64_t arena_cap, int64_t* arena_n,
+                            int32_t* hist, int32_t* flags, const ConfusionArgs* cm, void* workspace, size_t workspace_bytes,
+                            void* stream) {
   ETB_CHECK_ARG(det && det_cnt && img_meta && iouv && arena_conf && arena_cls && arena_tp && arena_n && hist && flags && workspace);
   ETB_CHECK_ARG(B > 0 && max_det > 0 && det_ld >= 6 && nt >= 0 && (targets || nt == 0) && H > 0 && W > 0 && nc > 0);
   ETB_CHECK_ARG(T > 0 && T <= VAL_MAX_T && arena_cap >= 0);
@@ -166,6 +175,11 @@ extern "C" int etb_val_epoch_append(const float* det, const int32_t* det_cnt, in
   ETB_CHECK_LAUNCH();
   int rc = etb_val_process_batch(det_native, det_cnt, B, max_det, 6, labels, nt, iouv, T, correct, flags + 1, stream);
   if (rc != ETB_OK) return rc;
+  if (cm) {                                    // the rescaled rows and labels above: predn and labelsn of val.py:373
+    rc = etb_confusion_matrix(det_native, det_cnt, B, max_det, 6, labels, nt, cm->nc, cm->conf_thres, cm->iou_thres, cm->matrix, cm->flags,
+                              stream);
+    if (rc != ETB_OK) return rc;
+  }
   etb_launch(val_append_kernel, dim3(B), dim3(256), 0, st, det_native, det_cnt, max_det, correct, T, arena_conf, arena_cls, arena_tp,
              arena_cap, arena_n, flags);
   ETB_CHECK_LAUNCH();
@@ -176,6 +190,27 @@ extern "C" int etb_val_epoch_append(const float* det, const int32_t* det_cnt, in
     if (rc != ETB_OK) return rc;
   }
   return ETB_OK;
+}
+
+extern "C" int etb_val_epoch_append(const float* det, const int32_t* det_cnt, int32_t B, int32_t max_det, int32_t det_ld,
+                                    const float* img_meta, const float* targets, int32_t nt, int32_t H, int32_t W, int32_t single_cls,
+                                    const float* iouv, int32_t T, int32_t nc, float* arena_conf, float* arena_cls, uint16_t* arena_tp,
+                                    int64_t arena_cap, int64_t* arena_n, int32_t* hist, int32_t* flags, void* workspace,
+                                    size_t workspace_bytes, void* stream) {
+  return val_epoch_append(det, det_cnt, B, max_det, det_ld, img_meta, targets, nt, H, W, single_cls, iouv, T, nc, arena_conf, arena_cls,
+                          arena_tp, arena_cap, arena_n, hist, flags, nullptr, workspace, workspace_bytes, stream);
+}
+
+extern "C" int etb_val_epoch_append_confusion(const float* det, const int32_t* det_cnt, int32_t B, int32_t max_det, int32_t det_ld,
+                                              const float* img_meta, const float* targets, int32_t nt, int32_t H, int32_t W,
+                                              int32_t single_cls, const float* iouv, int32_t T, int32_t nc, float* arena_conf,
+                                              float* arena_cls, uint16_t* arena_tp, int64_t arena_cap, int64_t* arena_n, int32_t* hist,
+                                              int32_t* flags, int32_t cm_nc, float cm_conf, float cm_iou, int64_t* cm_matrix,
+                                              int32_t* cm_flags, void* workspace, size_t workspace_bytes, void* stream) {
+  ETB_CHECK_ARG(cm_matrix && cm_flags && cm_nc > 0);
+  const ConfusionArgs cm = {cm_nc, cm_conf, cm_iou, cm_matrix, cm_flags};
+  return val_epoch_append(det, det_cnt, B, max_det, det_ld, img_meta, targets, nt, H, W, single_cls, iouv, T, nc, arena_conf, arena_cls,
+                          arena_tp, arena_cap, arena_n, hist, flags, &cm, workspace, workspace_bytes, stream);
 }
 
 // ---- epoch end: ap_per_class ---------------------------------------------------------------------------------------------

@@ -103,3 +103,88 @@ def ap_per_class(tp, conf, pred_cls, target_cls, plot=False, save_dir='.', names
     tc = target_cls.detach().cpu().numpy() if isinstance(target_cls, torch.Tensor) else np.asarray(target_cls)
     unique, n_l = np.unique(tc.astype(np.float64).reshape(-1), return_counts=True)
     return ap_from_device(conf_t, cls_t, pack_tp_bits(tp_t), n, T, unique, n_l)
+
+
+class ConfusionMatrix:
+    """utils/metrics.py:129-204 with the reference's surface; process_batch runs on the device (etb_confusion_matrix,
+    csrc/val.cu) and adds into an int64 count matrix there, without a host sync.  `matrix` reads it back as the reference's
+    float64 [nc+1, nc+1] (rows: predicted class, columns: true class, index nc: background).  A ValEpoch given this object
+    (val.run(..., confusion_matrix=cm)) adds every validation batch into it the same way.
+
+    Matches are decided by fp32 IoU; on an exact IoU tie the later label, then the later detection wins (the order numpy's
+    argsort()[::-1] gives where its sort is stable).  A class outside [0, nc) raises IndexError when the matrix is read:
+    numpy's indexing in the reference would raise for most of them, and take class nc or a negative class silently."""
+    host_plot = None        # the host application's ConfusionMatrix.plot, bound by efficientteacher_b200.bootstrap
+
+    def __init__(self, nc, conf=0.25, iou_thres=0.45):
+        self.nc, self.conf, self.iou_thres = int(nc), conf, iou_thres
+        if self.nc < 1:
+            raise ValueError("ConfusionMatrix: nc must be >= 1, got %d" % self.nc)
+        self.counts = None      # int64 [(nc+1)^2] on the device of the first batch
+        self.flags = None       # int32 [2]: an image with more than 1024 labels, a class outside [0, nc)
+        self.host = np.zeros((self.nc + 1, self.nc + 1))    # counts added on the host (the bootstrap's route for CPU tensors)
+
+    def buffers(self, device):
+        """(counts, flags) on `device`, allocated on first use"""
+        device = torch.device(device)
+        if self.counts is None:
+            self.counts = torch.zeros((self.nc + 1) ** 2, dtype=torch.int64, device=device)
+            self.flags = torch.zeros(2, dtype=torch.int32, device=device)
+        elif self.counts.device != device:
+            raise RuntimeError("ConfusionMatrix: counts live on %s, got a batch on %s" % (self.counts.device, device))
+        return self.counts, self.flags
+
+    def process_batch(self, detections, labels):
+        """one image: detections [N, >=6] (x1, y1, x2, y2, conf, cls) and labels [M, 5] (cls, x1, y1, x2, y2), CUDA tensors in
+        the same coordinate space.  fp16 rows are widened to fp32, exactly as torch promotes them against fp32 labels."""
+        _lib.require_cuda(detections, labels)
+        det = detections.float().contiguous()
+        if det.dim() != 2 or det.shape[1] < 6 or labels.dim() != 2 or labels.shape[1] != 5:
+            raise ValueError("ConfusionMatrix.process_batch: detections [N, 6] and labels [M, 5], got %s and %s"
+                             % (tuple(detections.shape), tuple(labels.shape)))
+        if det.shape[0] > 1024:
+            raise ValueError("ConfusionMatrix.process_batch: at most 1024 detections per image, got %d" % det.shape[0])
+        if det.shape[0] == 0:       # the reference counts every label as missed: one row below any conf threshold does that
+            det = torch.full((1, 6), float("-inf"), device=det.device)
+        counts, flags = self.buffers(det.device)
+        lab = torch.nn.functional.pad(labels.to(det.device, torch.float32), (1, 0))        # (img 0, cls, x1, y1, x2, y2)
+        _lib.check(_lib.lib().etb_confusion_matrix(_lib.ptr(det), None, 1, det.shape[0], det.shape[1], _lib.ptr(lab), lab.shape[0],
+                                                   self.nc, float(self.conf), float(self.iou_thres),
+                                                   _lib.ptr(counts), _lib.ptr(flags), _lib.stream_ptr(det.device)),
+                   "etb_confusion_matrix")
+
+    def check(self):
+        """raises if a batch overflowed or met a class outside [0, nc) (one read-back of the flags)"""
+        if self.flags is None:
+            return
+        f = self.flags.cpu().numpy()
+        if f[0]:
+            raise RuntimeError("ConfusionMatrix: an image carries more than 1024 labels (etb_confusion_matrix's limit)")
+        if f[1]:
+            raise IndexError("ConfusionMatrix: a class outside [0, %d) was to be counted" % self.nc)
+
+    @property
+    def matrix(self):
+        self.check()
+        m = self.host.copy()
+        if self.counts is not None:
+            m += self.counts.cpu().numpy().reshape(self.nc + 1, self.nc + 1)
+        return m
+
+    def reset(self):
+        self.host[:] = 0
+        if self.counts is not None:
+            self.counts.zero_()
+            self.flags.zero_()
+
+    def plot(self, normalize=True, save_dir='', names=()):
+        """the host application's drawing (seaborn) when the bootstrap has bound it; else the reference's warning line"""
+        if self.host_plot is None:
+            print('WARNING: ConfusionMatrix plot failure: no host plot bound (import efficientteacher_b200.bootstrap)')
+            return
+        self.host_plot(normalize=normalize, save_dir=save_dir, names=names)
+
+    def print(self):
+        m = self.matrix
+        for i in range(self.nc + 1):
+            print(' '.join(map(str, m[i])))

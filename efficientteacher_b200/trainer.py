@@ -196,16 +196,19 @@ class TrainerStep:
         return out
 
     # ---- end-of-epoch validation (val.run, native: val.py) ----
-    def _validate_model(self, model, dataloader, conf_thres, iou_thres, single_cls, names, half):
+    def _validate_model(self, model, dataloader, conf_thres, iou_thres, single_cls, names, half, confusion_matrix=None):
         from . import val
         return val.run({'nc': model.nc}, model=model, dataloader=dataloader, conf_thres=conf_thres, iou_thres=iou_thres,
-                       single_cls=single_cls, half=half, plots=False, val_ssod=hasattr(model, "det_8"), names=names or {})
+                       single_cls=single_cls, half=half, plots=False, val_ssod=hasattr(model, "det_8"), names=names or {},
+                       confusion_matrix=confusion_matrix)
 
-    def validate(self, dataloader, conf_thres=0.001, iou_thres=0.6, single_cls=False, names=None):
+    def validate(self, dataloader, conf_thres=0.001, iou_thres=0.6, single_cls=False, names=None, confusion_matrix=None):
         """trainer/trainer.py:451-464: validates ema.ema -> (results, maps, t).  As the reference's val.run leaves it, the
         EMA's floating state ends up rounded to fp16, here in place: no storage moves, so a captured step replayed afterwards
-        still reads and writes the EMA it was captured with."""
-        return self._validate_model(self.ema.ema, dataloader, conf_thres, iou_thres, single_cls, names, half=True)
+        still reads and writes the EMA it was captured with.  confusion_matrix: a metrics.ConfusionMatrix the validation adds
+        into (val.run)."""
+        return self._validate_model(self.ema.ema, dataloader, conf_thres, iou_thres, single_cls, names, half=True,
+                                    confusion_matrix=confusion_matrix)
 
     # the single ModelEMA of the supervised and the burn-in step, as graph B runs it
     def _ema_update_dev(self, scalars_dev):
@@ -614,18 +617,20 @@ class SSODTrainerStep(TrainerStep):
     def reset_graph(self):
         self._graph = None
 
-    def validate(self, dataloader, conf_thres=0.001, iou_thres=0.6, single_cls=False, names=None):
+    def validate(self, dataloader, conf_thres=0.001, iou_thres=0.6, single_cls=False, names=None, confusion_matrix=None):
         """ssod_trainer.py:335-383: the student, then the teacher of the current phase (semi_ema.ema after the hand-over,
         ema.ema during burn-in) -> (results, maps, t, cls_thr) of the teacher and the student's results.  The reference
         validates a deepcopy of the student only to spare it the fp16 rounding; here the student is validated in place
-        without rounding (same numbers) and put back in training mode.  The teacher is rounded in place (TrainerStep.validate)."""
+        without rounding (same numbers) and put back in training mode.  The teacher is rounded in place (TrainerStep.validate).
+        confusion_matrix: a metrics.ConfusionMatrix the teacher's validation adds into."""
         training = self.model.training
         try:
             student = self._validate_model(self.model, dataloader, conf_thres, iou_thres, single_cls, names, half=False)
         finally:
             self.model.train(training)
         teacher = self.semi_ema.ema if self.semi_ema is not None else self.ema.ema
-        results, maps, t, cls_thr = self._validate_model(teacher, dataloader, conf_thres, iou_thres, single_cls, names, half=True)
+        results, maps, t, cls_thr = self._validate_model(teacher, dataloader, conf_thres, iou_thres, single_cls, names, half=True,
+                                                         confusion_matrix=confusion_matrix)
         return results, maps, t, cls_thr, student[0]
 
     # ---- burn-in: trainer/ssod_trainer.py:295-317 (train_in_epoch), :421-456 / :490-533 -----------------------------

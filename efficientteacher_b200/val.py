@@ -6,8 +6,9 @@ in one launch -- returning the per-image tuples val.py appends to `stats`.
 
 run: the training-time val.run (a model and a dataloader given; plots, txt / json output, keypoints, model_post and
 augmented inference stay with the host application).  Every batch goes into a device-resident ValEpoch (etb_val_epoch_append:
-rescale, match and append without a host sync) and ap_per_class runs natively at the end (metrics.py).  The confusion matrix
-and the COCO json are not computed."""
+rescale, match and append without a host sync) and ap_per_class runs natively at the end (metrics.py).  With
+confusion_matrix= (a metrics.ConfusionMatrix) every batch is also added into the detection confusion matrix on the device.
+The COCO json is not computed."""
 import itertools
 from pathlib import Path
 
@@ -131,9 +132,11 @@ def _to_device(t, device, dtype=None):
 class ValEpoch:
     """The epoch's statistics (val.py:376 `stats`) in device memory: conf, class and correct bits of every detection in an
     arena that doubles when the host-side bound (images * max_det) outgrows it, and the label classes in an int32 histogram.
-    add() never waits for the device; finish() copies the counters back once and runs ap_per_class."""
+    add() never waits for the device; finish() copies the counters back once and runs ap_per_class.
+    confusion_matrix: a metrics.ConfusionMatrix that every batch is also added into (val.py:372-373), from the same rescaled
+    rows and labels, in the same launch sequence plus one kernel."""
 
-    def __init__(self, device, nc, iouv=None, single_cls=False, capacity=0):
+    def __init__(self, device, nc, iouv=None, single_cls=False, capacity=0, confusion_matrix=None):
         self.device, self.nc, self.single_cls = torch.device(device), int(nc), bool(single_cls)
         self.iouv = (torch.linspace(0.5, 0.95, 10) if iouv is None else torch.as_tensor(iouv)).to(self.device, torch.float32).contiguous()
         self.T = self.iouv.numel()
@@ -145,6 +148,9 @@ class ValEpoch:
         self.cap = self.bound = 0
         self.conf = self.cls = self.tp = None
         self.seen = self.n_labels = 0
+        self.cm = confusion_matrix
+        if self.cm is not None:
+            self.cm.buffers(self.device)
         self._grow(capacity)
 
     def _grow(self, need):
@@ -174,11 +180,17 @@ class ValEpoch:
         nt = tg.shape[0]
         lib = _lib.lib()
         ws = _ws.workspace("val_epoch", lib.etb_val_epoch_append_workspace_bytes(B, max_det, nt, self.T), self.device)
-        _lib.check(lib.etb_val_epoch_append(_lib.ptr(det), _lib.ptr(det_cnt), B, max_det, ld, _lib.ptr(meta), _lib.ptr(tg), nt,
-                                            int(img_hw[0]), int(img_hw[1]), int(self.single_cls), _lib.ptr(self.iouv), self.T, self.nc,
-                                            _lib.ptr(self.conf), _lib.ptr(self.cls), _lib.ptr(self.tp), self.cap, _lib.ptr(self.n_dev),
-                                            _lib.ptr(self.hist), _lib.ptr(self.flags), _lib.ptr(ws), ws.numel(),
-                                            _lib.stream_ptr(self.device)), "etb_val_epoch_append")
+        args = (_lib.ptr(det), _lib.ptr(det_cnt), B, max_det, ld, _lib.ptr(meta), _lib.ptr(tg), nt, int(img_hw[0]), int(img_hw[1]),
+                int(self.single_cls), _lib.ptr(self.iouv), self.T, self.nc, _lib.ptr(self.conf), _lib.ptr(self.cls), _lib.ptr(self.tp),
+                self.cap, _lib.ptr(self.n_dev), _lib.ptr(self.hist), _lib.ptr(self.flags))
+        tail = (_lib.ptr(ws), ws.numel(), _lib.stream_ptr(self.device))
+        if self.cm is None:
+            _lib.check(lib.etb_val_epoch_append(*args, *tail), "etb_val_epoch_append")
+        else:
+            cm = self.cm
+            counts, cm_flags = cm.buffers(self.device)
+            _lib.check(lib.etb_val_epoch_append_confusion(*args, cm.nc, float(cm.conf), float(cm.iou_thres), _lib.ptr(counts),
+                                                          _lib.ptr(cm_flags), *tail), "etb_val_epoch_append_confusion")
         self._keep = (meta, tg)       # the pinned staging buffers stay alive until the next batch
         self.seen += B
         self.n_labels += nt
@@ -192,6 +204,8 @@ class ValEpoch:
             raise RuntimeError("ValEpoch: an image carries more than 1024 labels (etb_val_process_batch's limit)")
         if hist[self.nc]:
             raise IndexError("ValEpoch: %d labels have a class outside [0, %d)" % (hist[self.nc], self.nc))
+        if self.cm is not None:
+            self.cm.check()
         nt = hist[:self.nc]
         if not flags[0]:
             return False, nt, None
@@ -295,11 +309,13 @@ def val_step(model, img, targets, shapes, epoch, conf_thres=0.001, iou_thres=0.6
 def run(data, weights=None, batch_size=32, imgsz=640, conf_thres=0.001, iou_thres=0.6, task='val', device='', single_cls=False,
         augment=False, verbose=False, save_txt=False, save_hybrid=False, save_conf=False, save_json=False, project=None, name='exp',
         exist_ok=False, half=True, model=None, dataloader=None, save_dir=Path(''), plots=True, callbacks=None, compute_loss=None,
-        model_post=None, eval_num=-1, cfg=None, val_ssod=False, num_points=0, val_kp=False, val_dp1000=False, dnn=False, names={}):
+        model_post=None, eval_num=-1, cfg=None, val_ssod=False, num_points=0, val_kp=False, val_dp1000=False, dnn=False, names={},
+        confusion_matrix=None):
     """val.py:149-465, the training-time call: returns ((mp, mr, map50, map, 0, 0, 0), maps, t[, cls_thr]).  The loss terms
     are zero as in the reference (its compute_loss branch is unreachable: `outputs is not list` always holds).  t is ms per
     image for (pre-process, inference, NMS), timed with CUDA events.  With half=True the model's floating state is rounded
-    to fp16 in place (what model.half(); model.float() leaves); the model is left in eval()."""
+    to fp16 in place (what model.half(); model.float() leaves); the model is left in eval().  confusion_matrix (native only,
+    a metrics.ConfusionMatrix): every image with NMS rows and labels is added into it, as val.py:372-373 does with plots=True."""
     why = run_unsupported(model=model, dataloader=dataloader, plots=plots, save_txt=save_txt, save_hybrid=save_hybrid,
                           save_json=save_json, num_points=num_points, model_post=model_post, augment=augment)
     if why:
@@ -317,7 +333,7 @@ def run(data, weights=None, batch_size=32, imgsz=640, conf_thres=0.001, iou_thre
     per_image = _registered(callbacks, 'on_val_image_end')
     s = ('%20s' + '%11s' * 6) % ('Class', 'Images', 'Labels', 'P', 'R', 'mAP@.5', 'mAP@.5:.95')
     print(s)
-    epoch = ValEpoch(device, nc, iouv, single_cls)
+    epoch = ValEpoch(device, nc, iouv, single_cls, confusion_matrix=confusion_matrix)
     stream = torch.cuda.current_stream(device)
     events = []
     for batch_i, (img, targets, paths, shapes) in enumerate(dataloader):

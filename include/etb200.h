@@ -426,6 +426,26 @@ int etb_val_epoch_append(const float* det, const int32_t* det_cnt, int32_t B, in
                          const float* iouv, int32_t T, int32_t nc, float* arena_conf, float* arena_cls, uint16_t* arena_tp,
                          int64_t arena_cap, int64_t* arena_n, int32_t* hist, int32_t* flags, void* workspace,
                          size_t workspace_bytes, void* stream);
+/* etb_val_epoch_append, and the same batch also added into the confusion matrix cm_matrix [(cm_nc+1)^2] int64 from the rows
+ * and labels it rescaled (etb_confusion_matrix with conf cm_conf, IoU cm_iou; its flags go to cm_flags[2]).  One rescale;
+ * one launch more than etb_val_epoch_append. */
+int etb_val_epoch_append_confusion(const float* det, const int32_t* det_cnt, int32_t B, int32_t max_det, int32_t det_ld,
+                                   const float* img_meta, const float* targets, int32_t nt, int32_t H, int32_t W, int32_t single_cls,
+                                   const float* iouv, int32_t T, int32_t nc, float* arena_conf, float* arena_cls, uint16_t* arena_tp,
+                                   int64_t arena_cap, int64_t* arena_n, int32_t* hist, int32_t* flags, int32_t cm_nc, float cm_conf,
+                                   float cm_iou, int64_t* cm_matrix, int32_t* cm_flags, void* workspace, size_t workspace_bytes,
+                                   void* stream);
+
+/* the detection confusion matrix (utils/metrics.py:129-186 ConfusionMatrix.process_batch), all images of a batch in one
+ * launch: det [B][max_det][det_ld>=6] fp32 rows (x1,y1,x2,y2,conf,cls) in the labels' coordinate space, det_cnt [B] (NULL:
+ * max_det rows per image); labels [nt][6] fp32 (img,cls,x1,y1,x2,y2).  Rows with conf > conf_thres are matched to labels
+ * class-agnostically at IoU > iou_thres, one label per detection and one detection per label by descending IoU (ties: the
+ * later label, then the later detection), and the counts are ADDED into matrix [(nc+1)^2] int64, row = predicted class,
+ * column = true class, nc = background.  As val.py calls it, an image with no row or no label adds nothing.  flags[0] = 1 if
+ * an image carries more than 1024 labels; flags[1] = 1 if a class to be counted (truncated like Tensor.int()) is outside
+ * [0, nc): it is not counted. */
+int etb_confusion_matrix(const float* det, const int32_t* det_cnt, int32_t B, int32_t max_det, int32_t det_ld, const float* labels,
+                         int32_t nt, int32_t nc, float conf_thres, float iou_thres, int64_t* matrix, int32_t* flags, void* stream);
 
 /* numeric core of ap_per_class (utils/metrics.py:22-126) over n rows conf [n] fp32, pred_cls [n] fp32, tp [n] uint16 (bit t =
  * true positive at IoU column t, T <= 16).  cls_slot [ncls_table]: the slot (0..nu-1, in ascending class order) of every
